@@ -1,10 +1,15 @@
 #!/usr/bin/env python
-"""bench.py — registrations/s of the kinematic-icp hot path on B200 (BASELINE.json metric).
+"""bench.py — registrations/s of the kinematic-icp hot path on H100 (BASELINE.json metric).
 
 A "step" is one full KinematicRegistration::ComputeRobotMotion (prior -> converged or max-iteration pose) of the
 OS1-128-shape synthetic scan (~262 k points) against the 1 M-point voxel map (BASELINE.json configs[3], "cfg4").
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload 1..4] [--mode sharded|replicas]
+                    [--dump-outputs DIR]
+
+--dump-outputs DIR writes what the last timed registration returned to its caller (the kicp_reg_result: pose, per-iteration
+sums and increments, beta, last |dx|, iteration count, status) as DIR/<name>.npy in float64.  The workload is generated from
+fixed seeds, so two builds run with the same arguments can be compared output for output.
 
 N > 1 is launched by torchrun, one rank per GPU.  In `sharded` mode (default, the north-star layout) the scan's
 points are split by contiguous index range, the map is replicated, and every IRLS iteration ends with one exchange of
@@ -29,7 +34,7 @@ for _p in (ROOT, os.path.join(ROOT, "kinematic-icp_b200", "python")):
 
 METRIC = "scans/sec (full ICP)"
 UNIT = "scans/s"
-L2_FLUSH_BYTES = 256 << 20  # > 126 MB L2
+L2_FLUSH_BYTES = 256 << 20  # > 50 MB L2 (H100)
 
 
 def parse_args():
@@ -47,7 +52,22 @@ def parse_args():
     ap.add_argument("--sustained", type=int, default=1000,
                     help="N = 1: registrations of the back-to-back run reported under `sustained` (0 = skip)")
     ap.add_argument("--no-flush", action="store_true", help="diagnostic only: keep L2 warm between steps")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the result of the last timed registration as DIR/<name>.npy (float64)")
+    args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    return args
+
+
+def dump_outputs(d, r):
+    """The kicp_reg_result a caller of the timed path receives, one float64 .npy per field (sums / dx: the iterations run)."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    arrays = {"pose": r.pose_np(), "sums": r.sums_np(), "dx": r.dx_np(), "beta": [r.beta], "last_dx_norm": [r.last_dx_norm],
+              "iterations": [r.iterations], "status": [r.status]}
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), np.asarray(a, dtype=np.float64))
 
 
 def workload_config(w, extra=None):
@@ -278,14 +298,15 @@ def sha256_file(path):
 
 
 def measure_l2_bandwidth(ctx):
-    """Read bandwidth of an L2-resident buffer on this GPU (the ceiling of a path whose working set lives in L2): 48 MiB read
-    40 times by one grid-stride launch with 128-bit loads (kicp_debug_l2_read_bandwidth), CUDA events, best of 3."""
+    """Read bandwidth of an L2-resident buffer on this GPU (the ceiling of a path whose working set lives in L2): 24 MiB (half
+    of the H100's 50 MB L2) read 40 times by one grid-stride launch with 128-bit loads (kicp_debug_l2_read_bandwidth), CUDA
+    events, best of 3."""
     import ctypes as C
     from kinematic_icp_b200 import _capi
     L = _capi.lib()
     L.kicp_debug_l2_read_bandwidth.argtypes = [C.c_void_p, C.c_uint64, C.c_int32, C.POINTER(C.c_double)]
     out = C.c_double()
-    st = L.kicp_debug_l2_read_bandwidth(ctx.h, 48 << 20, 40, C.byref(out))
+    st = L.kicp_debug_l2_read_bandwidth(ctx.h, 24 << 20, 40, C.byref(out))
     return float(out.value) if st == 0 else None
 
 
@@ -472,7 +493,8 @@ def main():
         timing = ctx.last_timing()  # CTA 0 of this rank, last registration: [pass][windows, barrier wait, reduce(+exchange), solve] ns
         jobs = world if (world > 1 and not sharded) else 1  # replicas: every rank finishes its own registrations
         out = {"value": jobs * args.steps / (total_ms * 1e-3), "ms_per_step": total_ms / args.steps, "prof": prof,
-               "launches": launches, "result": results[args.warmup], "n_local": hi - lo, "timing": timing}
+               "launches": launches, "result": results[args.warmup], "last_result": results[-1], "n_local": hi - lo,
+               "timing": timing}
 
         # e2e: host buffers through the public synchronous call, copies inside the timed region
         out_pose = np.empty(7)
@@ -613,7 +635,7 @@ def main():
         if os.path.exists(peaks_path):
             peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured copy)"
         else:
-            peak, peak_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+            peak, peak_src = 3350.0, "fallback 3.35 TB/s (H100 SXM data sheet, not measured)"
         prof = main_run["prof"]
         roofline = None
         if prof is not None and prof.assoc_launches > 0:
@@ -696,6 +718,8 @@ def main():
             line["replay"] = replay
         if cross_rank_identical is not None:
             line["cross_rank_identical"] = cross_rank_identical
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, main_run["last_result"])
         if replicas_run is not None:
             rv = replicas_run["e2e"]["pinned_f32"]
             line["replicas"] = {"value": replicas_run["value"], "unit": UNIT, "e2e": rv["value"], "scaling": "weak",

@@ -1,5 +1,5 @@
 /*
- * kicp.h — C ABI of the B200-native kinematic-icp registration hot path (libkicp_b200.so).
+ * kicp.h — C ABI of the H100-native kinematic-icp registration hot path (libkicp_b200.so).
  *
  * The reference (PRBonn/kinematic-icp @ 07c2851, v0.1.1) has no FFI: its hot path is a C++ value API
  * (SURVEY.md §8(b)).  This header is the boundary a binding for that path would bind; every entry point cites

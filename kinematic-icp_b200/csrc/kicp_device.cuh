@@ -54,7 +54,7 @@ __device__ __forceinline__ int voxel_coord(double x, double vs) { return (int)fl
 
 // DIVERGENCE SAFETY.  nvcc keeps loop-invariant kernel parameters (table mask, base pointers) in UNIFORM registers,
 // which are shared by the 32 lanes of a warp.  Inside a per-lane loop (a hash-probe chain, a voxel scan) that is only
-// sound while the sibling lanes wait at the reconvergence point; observed on sm_100a (cuda-gdb, DESIGN.md): siblings
+// sound while the sibling lanes wait at the reconvergence point; observed under cuda-gdb (DESIGN.md): siblings
 // ran past a BSYNC.RECONVERGENT, re-used the uniform register, and the lanes still probing read mask == 0 and spun on
 // slot 0 forever.  Two rules keep every kernel in this library safe (scripts/check_ur_loops.py verifies rule 1 on the
 // SASS):
@@ -79,11 +79,12 @@ __device__ __forceinline__ MapRegs map_regs(const MapView &m, MapView *shared_co
     return r;
 }
 
-// Same trick for a single 32-bit value (the table mask of the map-maintenance kernels): shared_words[32].
-__device__ __forceinline__ uint32_t lane_private(uint32_t v, uint32_t *shared_words) {
+// Same trick for a single scalar or pointer (the table mask of the map-maintenance kernels, ...): shared_words[32].
+template <class T>
+__device__ __forceinline__ T lane_private(T v, T *shared_words) {
     if (threadIdx.x < 32) shared_words[threadIdx.x] = v;
     __syncthreads();
-    return ((const volatile uint32_t *)shared_words)[threadIdx.x & 31];
+    return ((const volatile T *)shared_words)[threadIdx.x & 31];
 }
 
 // Read-only probe (no concurrent writers): returns the slot's meta word, or KICP_SLOT_EMPTY when absent.

@@ -52,7 +52,7 @@ struct kicp_scan_args {
 
 struct kicp_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t stream = nullptr;
     int64_t launches = 0;
     // registration scratch

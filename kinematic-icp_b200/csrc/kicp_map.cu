@@ -245,8 +245,8 @@ static int map_rebuild_table(kicp_map *m, uint32_t nslots) {
 }
 
 // All of a map's device storage is ONE allocation (the slab), carved into the arrays below for a capacity of `ncap` voxels.
-// Steady-state frames therefore never call cudaMalloc/cudaFree (measured: a growth event costs 0.4 - 240 ms on the B200
-// boxes, a steady-state Update 0.1 ms; profiles/r01_replay.md); growth doubles the capacity and migrates the contents.
+// Steady-state frames therefore never call cudaMalloc/cudaFree (a growth event costs far more than a steady-state Update);
+// growth doubles the capacity and migrates the contents.
 static int map_alloc_storage(kicp_map *m, uint32_t ncap) {
     kicp_ctx *c = m->ctx;
     const uint32_t slots_cap = std::max<uint32_t>(next_pow2((uint64_t)ncap * 4), 1024u);

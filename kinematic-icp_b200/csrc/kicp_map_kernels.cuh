@@ -134,7 +134,15 @@ __global__ void k_add_find_or_create(MapRW m, const double *__restrict__ xyz, in
 __global__ void k_add_commit(MapRW m, const double *__restrict__ xyz_t, const int32_t *__restrict__ pend_next,
                              uint32_t *counters, const int32_t *__restrict__ touched, double map_resolution) {
     __shared__ uint32_t s_mask[32];
-    const uint32_t tmask = lane_private(m.mask, s_mask);  // divergence safety, see kicp_device.cuh
+    __shared__ const double *s_xyz[32];
+    __shared__ double *s_pts[32];
+    __shared__ double s_res[32];
+    // divergence safety, see kicp_device.cuh (sm_90a keeps the two point arrays and map_resolution in uniform registers inside
+    // the replay loop otherwise)
+    const uint32_t tmask = lane_private(m.mask, s_mask);
+    xyz_t = lane_private(xyz_t, s_xyz);
+    m.pts = lane_private(m.pts, s_pts);
+    map_resolution = lane_private(map_resolution, s_res);
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= counters[1]) return;
     const uint32_t b = (uint32_t)touched[t];

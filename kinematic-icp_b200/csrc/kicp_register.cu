@@ -19,7 +19,7 @@
 //              a stage's tasks form one owner-major stream in the reference's visiting order, processed 32 at a time;
 //   lines      a found voxel's points are one contiguous run of 32-byte records, 4 per 128-byte line.  The lines of a stage
 //              are described in a per-warp buffer and evaluated in full rounds: a quad (4 lanes) takes one line, each lane
-//              loads ONE point with a single 256-bit load (a warp instruction touches 8 whole lines), KR_G rounds in flight;
+//              loads ONE point (a 128-bit and a 64-bit load: a warp instruction touches 8 lines), KR_G rounds in flight;
 //   reduction  the quad's minimum (two shuffles) goes to shared memory; every lane, as an owner, then scans the minima of
 //              its own lines in visiting order with the reference's rule (strict <, compared as norms: first minimum wins) and
 //              finally re-evaluates the winning line (pinned arithmetic) to name the point.  No atomics.
@@ -50,11 +50,11 @@
 using namespace kicp_dev;
 
 #ifndef KR_WARPS
-#define KR_WARPS 10                   // warps per CTA (measured: 2 x 10 warps per SM beat 2 x 8 and 3 x 8)
+#define KR_WARPS 10                   // warps per CTA (2 x 10 warps per SM; 64 K registers and 228 KB of shared memory per SM)
 #endif
 #define KR_THREADS (KR_WARPS * 32)
 #ifndef KR_MINB
-#define KR_MINB 2                     // resident CTAs per SM the kernel is compiled for (measured: the larger L1 beats more warps)
+#define KR_MINB 2                     // resident CTAs per SM the kernel is compiled for (a larger L1 rather than more warps)
 #endif
 #ifndef KR_LCAP
 #define KR_LCAP 192                   // lines the per-warp buffer holds (a batch of 32 tasks adds at most 160 at 20 points per voxel)
@@ -139,14 +139,17 @@ __device__ __forceinline__ unsigned long long ld_relaxed_sys_u64(const unsigned 
     return v;
 }
 #endif
-// one stored map point {x, y, z, pad}: a single 256-bit load (LDG.E.256, sm_100)
+// one stored map point {x, y, z, pad}, a 32-byte record in one 32-byte sector: x, y with one 128-bit load, z with a 64-bit one
+// (sm_90 has no 256-bit load; the pad is never read)
 struct __align__(32) Point4 {
     double x, y, z, w;
 };
 #ifndef KR_EMU
 __device__ __forceinline__ Point4 ld_point(const double *p) {
     Point4 r;
-    asm volatile("ld.global.nc.v4.f64 {%0, %1, %2, %3}, [%4];" : "=d"(r.x), "=d"(r.y), "=d"(r.z), "=d"(r.w) : "l"(p));
+    asm volatile("ld.global.nc.v2.f64 {%0, %1}, [%2];" : "=d"(r.x), "=d"(r.y) : "l"(p));
+    asm volatile("ld.global.nc.f64 %0, [%1];" : "=d"(r.z) : "l"(p + 2));
+    r.w = 0.0;
     return r;
 }
 #endif
@@ -694,7 +697,7 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                         // ---------------------------------------------------- evaluate the buffered lines
                         KR_PROF(3)
                         for (int r0 = 0; r0 < fill; r0 += 8 * KR_G) {
-                            // a quad takes a line, a lane ONE point of it; KR_G independent 256-bit loads per lane in flight
+                            // a quad takes a line, a lane ONE point of it; KR_G independent point loads per lane in flight
                             unsigned own[KR_G], gix[KR_G];
                             unsigned hasm = 0;
 #pragma unroll

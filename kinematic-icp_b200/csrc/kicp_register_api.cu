@@ -229,7 +229,7 @@ static int enqueue_registration(kicp_map *m, const kicp_scan *scan, const double
             if (pr) KICP_CUDA(cudaEventRecord(e1, c->stream));
             // The frame's chunks go out AFTER the launch: the kernel is already resident and takes every chunk as its flag rises, and the
             // host-side cost of the copies (for pageable memory the driver stages each of them on this thread) no longer delays the
-            // launch — same box, pageable float32: 2 736 instead of 2 390 scans/s end to end, float64 1 952 instead of 1 771.
+            // launch, which matters most to a caller with pageable buffers.
             // (A copy that fails here leaves the kernel to its wait timeout; the call drains both streams and reports the error.)
             if (ka.up.flags != nullptr) KICP_TRY(issue_chunks(c, *host_upload));
             if (dbg) {

@@ -1,4 +1,4 @@
-"""B200-native kinematic-icp registration hot path — host-side mirror of the reference's C++ interface.
+"""H100-native kinematic-icp registration hot path — host-side mirror of the reference's C++ interface.
 
 The classes keep the reference's names and argument meaning:
 

@@ -1,7 +1,6 @@
-"""Generates tests/golden/*.npz from the REFERENCE'S OWN sources compiled here (oracle/_ref/libkicp_ref.so =
-/root/reference/cpp/kinematic_icp/{registration/Registration.cpp, correspondence_threshold/CorrespondenceThreshold.cpp,
-pipeline/KinematicICP.cpp} built against header shims, see oracle/Makefile).  Run in the authoring container only
-(/root/reference does not exist on the GPU box):
+"""Generates tests/golden/*.npz from the REFERENCE'S OWN sources (oracle/_ref/libkicp_ref.so = the reference checkout's
+cpp/kinematic_icp/{registration/Registration.cpp, correspondence_threshold/CorrespondenceThreshold.cpp, pipeline/KinematicICP.cpp}
+built against header shims, see oracle/Makefile).  Run where a reference checkout exists:
 
     python tests/golden/make_golden.py
 
@@ -65,9 +64,37 @@ def pipeline_fixture():
     np.savez_compressed(os.path.join(HERE, "pipeline_seq.npz"), **out)
 
 
+def ref_cfg2_threads_fixture():
+    """Registration.cpp on workload cfg2 with 1 and 3 threads (tests/test_golden_cpu.py::test_oracle_matches_reference_build_live)."""
+    w = W.Workload(2)
+    _, _, pts = w.map.export_voxels()
+    rm = ko.RefMap(w.voxel_size, w.max_range, w.max_points_per_voxel)
+    rm.add_points(pts)
+    threads = [1, 3]
+    poses = [rm.register(w.scan, w.last_pose, w.rel_odom, w.tau, threads=t) for t in threads]
+    np.savez_compressed(os.path.join(HERE, "ref_cfg2_threads.npz"), threads=np.array(threads), poses=np.array(poses))
+    print("ref_cfg2_threads", poses[0])
+
+
+def ref_fuzz_fixture():
+    """Registration.cpp, one thread, on the random scenes of tests/test_golden_cpu.py::fuzz_cases."""
+    sys.path.insert(0, os.path.dirname(HERE))
+    from test_golden_cpu import fuzz_cases
+    poses = []
+    for _, vs, cap, stored, scan, last, odom, tau, kw in fuzz_cases(ko):
+        rm = ko.RefMap(vs, 100.0, cap)
+        rm.add_points(stored)  # voxel-grouped insertion order reproduces the same content
+        assert rm.num_points() == len(stored)
+        poses.append(rm.register(scan, last, odom, tau, threads=1, **kw))
+    np.savez_compressed(os.path.join(HERE, "ref_fuzz.npz"), poses=np.array(poses))
+    print("ref_fuzz", len(poses), "cases")
+
+
 if __name__ == "__main__":
     assert ko.ref_available(), "build oracle/_ref first: make -C oracle ref"
     registration_fixture("reg_cfg1", 1)
     registration_fixture("reg_cfg2_small", 2, M=30_000, n_az=450)
     threshold_fixture()
     pipeline_fixture()
+    ref_cfg2_threads_fixture()
+    ref_fuzz_fixture()

@@ -70,7 +70,8 @@ def test_downsample_order_modes_keep_the_same_points(oracle, workload):
     assert np.array_equal(ko.voxel_downsample(w.scan, 0.5), base)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/cpp/kinematic_icp"), reason="reference tree not present (GPU box)")
+@pytest.mark.skipif(not os.path.exists(os.path.join(os.path.dirname(GOLDEN), "..", "oracle", "_ref", "libkicp_ref.so")),
+                    reason="oracle/_ref (the reference's own sources, built where a reference checkout exists) not built")
 @pytest.mark.parametrize("deskew", [False, True])
 def test_trajectory_sensitivity_to_the_downsample_order(oracle, deskew):
     """The reference's own pipeline sources over the restated KISS-ICP, golden drive, with the down-sample emitting the recalled

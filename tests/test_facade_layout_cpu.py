@@ -2,7 +2,8 @@
 the reference's own pipeline/KinematicICP.hpp (with the oracle's header shims for the libraries that are absent offline) and
 against this repo's facade header — using aggregate initialisation of Config, assignment of every field by name and a
 subclass that reaches the five protected members by name; the two builds must report the same sizeof / offsetof of Config.
-Where /root/reference is absent (the GPU box) the facade build is checked against the recorded numbers."""
+The facade build is always checked against the numbers recorded from the reference build; the reference header itself is
+compiled too when KICP_REFERENCE_DIR names a reference checkout."""
 import os
 import subprocess
 import tempfile
@@ -10,7 +11,7 @@ import tempfile
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference/cpp"
+REF = os.path.join(os.environ.get("KICP_REFERENCE_DIR", ""), "cpp")
 TU = r"""
 #include <cstddef>
 #include <cstdio>

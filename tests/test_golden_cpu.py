@@ -38,23 +38,20 @@ def test_threshold_matches_reference_golden(oracle):
         assert th.compute() == tau
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/cpp/kinematic_icp"), reason="reference tree not present (GPU box)")
 def test_oracle_matches_reference_build_live(oracle, workload):
-    """In the authoring container: the restatement against oracle/_ref (the reference's Registration.cpp) directly."""
+    """The restatement against the poses the reference's own Registration.cpp (oracle/_ref) returned on cfg2 with 1 and 3 threads
+    (tests/golden/ref_cfg2_threads.npz)."""
     ko = oracle
-    assert ko.ref_available()
+    z = np.load(os.path.join(GOLDEN, "ref_cfg2_threads.npz"))
     w = workload(2)
-    _, _, pts = w.map.export_voxels()
-    rm = ko.RefMap(w.voxel_size, w.max_range, w.max_points_per_voxel)
-    rm.add_points(pts)
-    for thr in (1, 3):
-        pr = rm.register(w.scan, w.last_pose, w.rel_odom, w.tau, threads=thr)
-        po, _ = w.map.register(w.scan, w.last_pose, w.rel_odom, w.tau)
+    po, _ = w.map.register(w.scan, w.last_pose, w.rel_odom, w.tau)
+    for thr, pr in zip(z["threads"], z["poses"]):
         dt, ang = ko.pose_delta(pr, po)
-        assert dt < 1e-12 and ang < 1e-12
+        assert dt < 1e-12 and ang < 1e-12, (thr, dt, ang)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/cpp/kinematic_icp"), reason="reference tree not present (GPU box)")
+@pytest.mark.skipif(not os.path.exists(os.path.join(os.path.dirname(GOLDEN), "..", "oracle", "_ref", "libkicp_ref.so")),
+                    reason="oracle/_ref (the reference's own sources, built where a reference checkout exists) not built")
 def test_pipeline_golden_is_reproducible(oracle):
     """The committed pipeline fixture equals a fresh run of the reference's own pipeline sources (threads = 1)."""
     from oracle import sequences as S
@@ -67,20 +64,11 @@ def test_pipeline_golden_is_reproducible(oracle):
     assert np.array_equal(poses, z["deskew_poses"]) and np.array_equal(n_map, z["deskew_n_map"])
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/cpp/kinematic_icp"), reason="reference tree not present (GPU box)")
-def test_oracle_matches_reference_build_fuzz(oracle):
-    """Randomised pin of the restatement: small random scenes and random solver settings (0..25 iterations, adaptive / fixed
-    regularisation, gates from 5 cm to 3 m, empty scans), the oracle against the reference's own Registration.cpp (oracle/_ref,
-    one thread = the same summation order).  Same NaN pattern, poses within 1e-14 (most are bit-identical; the rest differ by
-    one rounding: the test wrapper rebuilds Sophus::SE3d from a pose7, whose constructor re-normalises the quaternion)."""
-    from oracle.workloads import unicycle as _unicycle
-    ko = oracle
+def fuzz_cases(ko):
+    """40 small random scenes and random solver settings (0..25 iterations, adaptive / fixed regularisation, gates from 5 cm to
+    3 m, empty scans), each as (oracle map, its voxel-grouped points, scan, last pose, odometry, tau, solver settings)."""
+    from oracle.workloads import unicycle
     rng = np.random.default_rng(20260923)
-    exact = 0
-
-    def unicycle(_, d, th):
-        return _unicycle(d, th)
-
     for case in range(40):
         vs = float(rng.choice([0.5, 1.0, 2.0]))
         cap = int(rng.choice([1, 5, 20]))
@@ -90,27 +78,37 @@ def test_oracle_matches_reference_build_fuzz(oracle):
         wall = np.c_[rng.uniform(-25, 25, n_map // 2), np.full(n_map // 2, 12.0) + 0.02 * rng.standard_normal(n_map // 2),
                      rng.uniform(0, 4, n_map // 2)]
         om = ko.OracleMap(vs, 100.0, cap)
-        rm = ko.RefMap(vs, 100.0, cap)
         pts = np.concatenate([ground, wall])
         om.add_points(pts)
         _, _, stored = om.export_voxels()
-        rm.add_points(stored)  # voxel-grouped insertion order reproduces the same content
-        assert rm.num_points() == om.num_points()
         last = ko.planar_pose(*rng.uniform(-3, 3, 2), rng.uniform(-3.1, 3.1))
-        true_rel = unicycle(ko, rng.uniform(0.0, 1.0), rng.uniform(-0.1, 0.1))
-        odom = unicycle(ko, rng.uniform(0.0, 1.1), rng.uniform(-0.12, 0.12))
+        true_rel = unicycle(rng.uniform(0.0, 1.0), rng.uniform(-0.1, 0.1))
+        odom = unicycle(rng.uniform(0.0, 1.1), rng.uniform(-0.12, 0.12))
         n_scan = int(rng.integers(0, 3000))
         world = pts[rng.integers(0, len(pts), n_scan)] + 0.01 * rng.standard_normal((n_scan, 3))
         scan = ko.se3_transform(ko.se3_inverse(ko.se3_compose(last, true_rel)), world) if n_scan else np.zeros((0, 3))
         tau = float(rng.choice([0.05, 0.3, 1.0, 3.0]))
         kw = dict(max_iter=int(rng.choice([0, 1, 3, 10, 25])), conv=float(rng.choice([1e-3, 1e-6, 1e-1])),
                   adaptive=bool(rng.integers(0, 2)), fixed_reg=float(rng.choice([0.0, 0.1, 10.0])))
+        yield om, vs, cap, stored, scan, last, odom, tau, kw
+
+
+def test_oracle_matches_reference_build_fuzz(oracle):
+    """Randomised pin of the restatement: the oracle on the scenes of fuzz_cases against the poses the reference's own
+    Registration.cpp (oracle/_ref, one thread = the same summation order) returned for them (tests/golden/ref_fuzz.npz).  Same NaN
+    pattern, poses within 1e-14 (most are bit-identical; the rest differ by one rounding: the test wrapper rebuilds Sophus::SE3d
+    from a pose7, whose constructor re-normalises the quaternion)."""
+    ko = oracle
+    ref = np.load(os.path.join(GOLDEN, "ref_fuzz.npz"))["poses"]
+    exact = 0
+    for case, (om, _, _, stored, scan, last, odom, tau, kw) in enumerate(fuzz_cases(ko)):
+        assert om.num_points() == len(stored)
         po, _ = om.register(scan, last, odom, tau, **kw)
-        pr = rm.register(scan, last, odom, tau, threads=1, **kw)
+        pr = ref[case]
         assert np.array_equal(np.isnan(po), np.isnan(pr)), (case, kw)
         if np.isnan(po).any():
             continue
         dt, ang = ko.pose_delta(po, pr)
         assert dt < 1e-14 and ang < 1e-14, (case, kw, dt, ang)
         exact += int(np.array_equal(po, pr))
-    assert exact >= 20
+    assert case == 39 and exact >= 20
