@@ -65,8 +65,8 @@ struct kicp_ctx {
     int collect_stats = 0;  // option "stats": count probes / candidate points / lines on the device
     int spin_timeout_ms = 20000;  // bound of every device-side wait (upload flags, peers of the fused exchange)
     // nearest-neighbour cache of the persistent kernel (one entry per scan point, carried from pass to pass)
-    unsigned int *d_nn_g = nullptr, *d_nn_g2 = nullptr, *d_todo = nullptr;
-    float *d_nn_l = nullptr, *d_nn_seed = nullptr;
+    unsigned int *d_nn_g = nullptr, *d_nn_g2 = nullptr, *d_todo = nullptr, *d_todo2 = nullptr;
+    float *d_nn_l = nullptr;
     int64_t nn_cap = 0;
     int nn_cache = 1;  // option "nn_cache"
     int frame_sync = 0;       // option "frame_sync": 1 = kicp_register_frame reads the survivor counts back mid-frame (legacy order)

@@ -168,8 +168,8 @@ extern "C" int kicp_ctx_destroy(kicp_ctx *ctx) {
     cudaFree(ctx->d_nn_g);
     cudaFree(ctx->d_nn_g2);
     cudaFree(ctx->d_nn_l);
-    cudaFree(ctx->d_nn_seed);
     cudaFree(ctx->d_todo);
+    cudaFree(ctx->d_todo2);
     cudaFree(ctx->d_prof_iters);
     cudaFree(ctx->d_scan_status);
     cudaFree(ctx->d_scan_ticket);

@@ -34,8 +34,9 @@
 // (a step into a neighbouring voxel brings one layer of voxels in: those lie beyond the far face of the new own voxel), so
 // min(|q' - g1|, |q' - g2|) < l - delta proves the nearer of the two is still THE strict nearest neighbour and the search is skipped.
 // The remaining points are compacted and searched (phase B) with |q' - g| as an exact pruning bound: the usual ones — few voxels
-// inside that bound — in ONE merged stage (front of the list, ordinary windows), the stragglers staged, in small windows of their
-// own (back of the list), so that no ordinary window walks through three stages for the sake of one lane.
+// inside that bound — in ONE merged stage, the stragglers staged, in small windows of their own, so that no ordinary window walks
+// through three stages for the sake of one lane.  Phase A sorts the merged ones into cost classes by task count; phase B deals the
+// class-ordered list to its windows, so every window gets the same share of each class and no window outlasts the others by much.
 #include <cfloat>
 #include <cmath>
 #include <cstddef>
@@ -60,13 +61,22 @@ using namespace kicp_dev;
 #define KR_LCAP 192                   // lines the per-warp buffer holds (a batch of 32 tasks adds at most 160 at 20 points per voxel)
 #endif
 #ifndef KR_G
-#define KR_G 2                        // line-rounds (of 8 lines = 32 points) in flight together (96 registers at 2 x 320 threads)
+#define KR_G 3                        // line-rounds (of 8 lines = 32 points) in flight together (96 registers at 2 x 320 threads)
 #endif
 #ifndef KR_MERGE_MAX
 #define KR_MERGE_MAX 19               // neighbour voxels a seeded point may bring into its single merged stage (20 tasks x 32 owners = KR_TCAP)
 #endif
 #ifndef KR_SLOWWIN
 #define KR_SLOWWIN 8                  // points per window of the staged stragglers of a later pass
+#endif
+// Cost classes of the points a later pass searches again: 0 = staged stragglers; 1, 2, 3 = one merged stage of >= KR_CLS_HEAVY,
+// >= KR_CLS_MID, fewer tasks (own voxel + the neighbour voxels inside the bound).
+#define KR_CLASSES 4
+#ifndef KR_CLS_HEAVY
+#define KR_CLS_HEAVY 8
+#endif
+#ifndef KR_CLS_MID
+#define KR_CLS_MID 4
 #endif
 #define KR_DBLMAX_BITS 0x7FEFFFFFFFFFFFFFull
 // Development aid (-DKR_PROFILE): per-phase cycle accounting of the window loop (lane 0 of every warp, clock64 deltas).
@@ -103,8 +113,11 @@ struct RegState {
     unsigned int exit_ctr;          // CTAs that have left the kernel; the last one zeroes the three counters
     unsigned int ticket;            // multi-launch path: last-CTA detection
     unsigned int a_arrive;          // warps that finished the certificate phase of a pass (monotonic inside a registration)
-    unsigned int todo_n[KICP_MAX_ITERATIONS];  // per pass: points whose neighbour has to be searched again (front of the list) ...
-    unsigned int slow_n[KICP_MAX_ITERATIONS];  // ... and those among them that need the staged search (back of the list)
+    union {  // per cost class and pass: points whose neighbour has to be searched again (arrival counters of the class lists)
+        unsigned int cls_n[KR_CLASSES][KICP_MAX_ITERATIONS];
+        // (the same counters by class name; the CPU test harness in tests/emu checks todo_n and slow_n)
+        struct { unsigned int slow_n[KICP_MAX_ITERATIONS], heavy_n[KICP_MAX_ITERATIONS], mid_n[KICP_MAX_ITERATIONS], todo_n[KICP_MAX_ITERATIONS]; };
+    };
     int abort;                      // a device-side wait gave up (status code); every CTA leaves after the current pass
     int *iters_out;                 // optional: where to publish the iteration count (profiling)
     double acc[8];                  // multi-launch path: JTJ00 JTJ01 JTJ11 JTr0 JTr1 N sum|r|^2 (unused)
@@ -160,7 +173,8 @@ __global__ void k_reg_init(RegState *st, RegArgs a) {
     pose_init(&st->pose, a);
     result_init(&st->result, &st->pose);
     st->ticket = 0, st->win_ctr = 0, st->arrive = 0, st->exit_ctr = 0, st->abort = 0, st->a_arrive = 0;
-    for (int k = 0; k < KICP_MAX_ITERATIONS; ++k) st->todo_n[k] = 0, st->slow_n[k] = 0;
+    for (int c = 0; c < KR_CLASSES; ++c)
+        for (int k = 0; k < KICP_MAX_ITERATIONS; ++k) st->cls_n[c][k] = 0;
     st->iters_out = a.iters_out;
     if (a.iters_out) *a.iters_out = 0;
     for (int k = 0; k < 8; ++k) st->acc[k] = 0.0;
@@ -268,12 +282,19 @@ __device__ __forceinline__ unsigned stage_mask(int stage, bool valid, double bou
 
 // A point that enters a later pass with `sd`, the distance to its previous neighbour at the new position, has an exact pruning bound
 // from the start: the neighbour voxels that survive it.  Evaluated identically by the certificate sweep (which sorts the point into
-// the list of one-stage searches if they are few) and by the search itself.
+// a cost class by their number) and by the search itself.
 __device__ __forceinline__ unsigned seeded_near_mask(double sd, double tau, double qx, double qy, double qz, int vx, int vy, int vz, double vs,
                                                      double &minpruned) {
     const double seed2 = sd * sd * (1.0 + 1e-6);
     const double bound = fmin(tau * tau, seed2) * (1.0 + 1e-6) + 1e-10;
     return stage_mask(1, true, bound, qx, qy, qz, vx, vy, vz, vs, minpruned) | stage_mask(2, true, bound, qx, qy, qz, vx, vy, vz, vs, minpruned);
+}
+
+// Entry `pos` of cost class c's list.  The four classes share two arrays of n entries, one class growing from each end, so the
+// lists come out class-ordered without knowing the class sizes in advance.
+__device__ __forceinline__ unsigned *class_entry(const KernelArgs &a, int n, int c, unsigned pos) {
+    unsigned *const base = (c == 0 || c == 3) ? a.todo : a.todo2;
+    return base + ((c & 1) ? pos : (unsigned)n - 1u - pos);
 }
 
 // gate, residual, Jacobian and the seven sums of one correspondence (Registration.cpp:75, 86-93, 110-118)
@@ -317,6 +338,7 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
     __shared__ double s_part[KR_WARPS][8];
     __shared__ double s_sum[8];
     __shared__ int s_flag[2];
+    __shared__ volatile int s_ncls[2];  // a later pass's search: points of the heavy and the middle class
 
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int quad = lane >> 2, sub = lane & 3;
@@ -430,34 +452,35 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                     if (haveg) accumulate(sm, lane, s_ps, c.x, c.y, c.z, qx, qy, qz, px, py);
                 }
                 // Everything else is searched again.  The old neighbour bounds that search if it is one of the new 27 voxels' points; with
-                // few neighbour voxels inside the bound the search is ONE merged stage (front of the list), else it is staged (back).
+                // few neighbour voxels inside the bound the search is ONE merged stage, else it is staged.  The point goes to the list
+                // of its cost class: staged, or by the tasks of its merged stage (its own voxel and the neighbours inside the bound).
                 const bool again = valid && !cert;
-                bool slow = false;
+                int cls = -1;
                 if (again) {
                     float seed = 3.0e38f;
                     if (haveg && abs(voxel_of(c.x, vs, inv_vs, a.pow2_voxel) - vx) <= 1 && abs(voxel_of(c.y, vs, inv_vs, a.pow2_voxel) - vy) <= 1 &&
                         abs(voxel_of(c.z, vs, inv_vs, a.pow2_voxel) - vz) <= 1)
                         seed = __double2float_ru(dn * (1.0 + 1e-7));
-                    a.nn_seed[i] = seed;
-                    slow = true;
+                    a.nn_l[i] = seed;  // (the search reads it from here and then writes the new certificate)
+                    cls = 0;
                     if (seed < 1.0e38f) {
                         double mp = DBL_MAX;
-                        slow = __popc(seeded_near_mask((double)seed, s_ps.tau, qx, qy, qz, vx, vy, vz, vs, mp)) > KR_MERGE_MAX;
+                        const int near = __popc(seeded_near_mask((double)seed, s_ps.tau, qx, qy, qz, vx, vy, vz, vs, mp));
+                        if (near <= KR_MERGE_MAX) cls = near + 1 >= KR_CLS_HEAVY ? 1 : near + 1 >= KR_CLS_MID ? 2 : 3;
                     }
                 }
-                const unsigned needf = __ballot_sync(FULL, again && !slow), needs = __ballot_sync(FULL, again && slow);
-                if (needf) {
-                    unsigned pos = 0;
-                    if (lane == 0) pos = atomicAdd(&st->todo_n[it], (unsigned)__popc(needf));
-                    pos = __shfl_sync(FULL, pos, 0) + (unsigned)__popc(needf & ((1u << lane) - 1u));
-                    if (again && !slow) a.todo[pos] = (unsigned)i;
+                // one arrival counter per class (lane k < KR_CLASSES bumps class k's): the lanes of a class take consecutive entries of its list
+                unsigned need = 0u, cnt = 0u;
+#pragma unroll
+                for (int k = 0; k < KR_CLASSES; ++k) {
+                    const unsigned m = __ballot_sync(FULL, cls == k);
+                    if (cls == k) need = m;
+                    if (lane == k) cnt = m;
                 }
-                if (needs) {
-                    unsigned pos = 0;
-                    if (lane == 0) pos = atomicAdd(&st->slow_n[it], (unsigned)__popc(needs));
-                    pos = __shfl_sync(FULL, pos, 0) + (unsigned)__popc(needs & ((1u << lane) - 1u));
-                    if (again && slow) a.todo[(unsigned)n - 1u - pos] = (unsigned)i;
-                }
+                unsigned pos = 0;
+                if (cnt) pos = atomicAdd(&st->cls_n[lane][it], (unsigned)__popc(cnt));
+                pos = __shfl_sync(FULL, pos, max(cls, 0)) + (unsigned)__popc(need & ((1u << lane) - 1u));
+                if (cls >= 0) *class_entry(a, n, cls, pos) = (unsigned)i;
             }
             KR_WLOG(1, t_iter0, gtime_ns(), 0, 0)
             // every CTA of the grid has to be through phase A before the list is complete
@@ -476,20 +499,21 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                     }
                 }
                 t_a2 = gtime_ns();
+                s_ncls[0] = (int)__ldcg(&st->cls_n[1][it]), s_ncls[1] = (int)__ldcg(&st->cls_n[2][it]);
             }
             __syncthreads();
         }
         const bool indirect = cache && it > 0u;
-        // points of the search phase: in pass 0 the whole frame; afterwards the uncertified ones — at the front of the list those
-        // that get by with ONE merged stage (the usual case), at its back the few that need the staged search
-        const int nfast = indirect ? (int)__ldcg(&st->todo_n[it]) : n;
-        const int nslow = indirect ? (int)__ldcg(&st->slow_n[it]) : 0;
+        // points of the search phase: in pass 0 the whole frame; afterwards the uncertified ones — those that get by with ONE merged
+        // stage (the usual case) in three cost classes, heaviest first, and the few that need the staged search
+        const int nfast = indirect ? (int)(__ldcg(&st->cls_n[1][it]) + __ldcg(&st->cls_n[2][it]) + __ldcg(&st->cls_n[3][it])) : n;
+        const int nslow = indirect ? (int)__ldcg(&st->cls_n[0][it]) : 0;
         // Window size of the phase.  A window is a chain of dependent steps whose length depends little on how many points it holds,
         // so full windows are the efficient unit; but when the whole phase fits ONE round of the grid, the points are spread evenly
         // over all warps (a small scan, the remainder of a later pass), and a phase of k rounds sizes its windows so that every warp
         // gets k of them (no last round that only part of the grid takes part in).  The staged stragglers of a later pass go into
-        // small windows of their own (KR_SLOWWIN points, handed out first): one of them inside an ordinary window would make all
-        // its 32 lanes walk through the three stages.
+        // small windows of their own (KR_SLOWWIN points, handed out first, and counted in the rounds): one of them inside an ordinary
+        // window would make all its 32 lanes walk through the three stages.
         const int P = (int)total_warps;
         const int nslowwin = (nslow + KR_SLOWWIN - 1) / KR_SLOWWIN;
         const int Pf = max(P - nslowwin, P / 2);  // warps left for the ordinary windows of a single-round phase
@@ -498,8 +522,8 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
             if (nfast <= 32 * Pf) {
                 wsz = max(1, (nfast + Pf - 1) / Pf);
             } else {
-                const int rounds = (nfast + 32 * P - 1) / (32 * P);
-                wsz = min(32, (nfast + rounds * P - 1) / (rounds * P));
+                const int rounds = (nfast + 32 * (P + nslowwin) - 1) / (32 * P);  // (a staged window takes a warp's turn)
+                wsz = min(32, (nfast + rounds * Pf - 1) / (rounds * Pf));
             }
         }
         // pass 0: the frame in KICP_UPLOAD_CHUNKS segments of `segpts` points (the host uploads it in exactly these pieces)
@@ -529,15 +553,15 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
             // ---------------------------------------------------------------- owners: q = T p and its voxel
             // The points of a phase are DEALT to its windows like cards (owner `lane` of window w = entry lane * windows + w): points
             // that are expensive to search (little or no map around them) sit next to each other in the scan and in the list, and a
-            // window made of them alone would outlast the phase.  Pass 0 deals inside each of the KICP_UPLOAD_CHUNKS segments the
-            // frame is uploaded in, so that a window still needs only its own chunk.
-            int slot, limit, seg_of_w = 0, wlanes = wsz;
-            bool from_back = false;
+            // window made of them alone would outlast the phase.  In a later pass the list is ordered by cost class, so every window
+            // gets the same share of each class: the windows of the phase cost about the same.  Pass 0 deals inside each of the
+            // KICP_UPLOAD_CHUNKS segments the frame is uploaded in, so that a window still needs only its own chunk.
+            int slot, limit, seg_of_w = 0, wlanes = wsz, cls = 0;
             if (indirect) {
-                if (w < nslowwin) {  // a small window of staged stragglers (back of the list)
-                    slot = lane * nslowwin + w, limit = nslow, wlanes = KR_SLOWWIN, from_back = true;
-                } else {
-                    slot = lane * nfastwin + (w - nslowwin), limit = nfast;
+                if (w < nslowwin) {  // a small window of staged stragglers
+                    slot = lane * nslowwin + w, limit = nslow, wlanes = KR_SLOWWIN;
+                } else {             // the one-stage classes, heaviest first
+                    slot = lane * nfastwin + (w - nslowwin), limit = nfast, cls = 1;
                 }
             } else {
                 const int sgi = min(w / segwin, KICP_UPLOAD_CHUNKS - 1), lw = w - sgi * segwin;
@@ -547,7 +571,13 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                 seg_of_w = sgi;
             }
             const bool valid = lane < wlanes && slot < limit;
-            const int pi = valid ? (indirect ? (int)__ldcg(&a.todo[from_back ? n - 1 - slot : slot]) : slot) : 0;  // the owner's scan point
+            int pi = valid ? slot : 0;  // the owner's scan point
+            if (indirect) {
+                int pos = slot;  // ... the entry `pos` of its class's list
+                if (cls == 1 && pos >= s_ncls[0]) pos -= s_ncls[0], cls = 2;
+                if (cls == 2 && pos >= s_ncls[1]) pos -= s_ncls[1], cls = 3;
+                pi = valid ? (int)__ldcg(class_entry(a, n, cls, (unsigned)pos)) : 0;
+            }
             if (PERSISTENT && a.up.flags != nullptr && it == 0u) {
                 // first pass over a frame that is still being uploaded: wait until this window's chunk has landed
                 const uint32_t *f = a.up.flags + seg_of_w;
@@ -569,7 +599,7 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                 double px = 0, py = 0, pz = 0;
                 if (valid) load_scan_point(a.scan, pi, px, py, pz);
                 if (indirect && valid) {
-                    const double sd = (double)__ldcg(&a.nn_seed[pi]);
+                    const double sd = (double)__ldcg(&a.nn_l[pi]);  // (the seed, left there by the certificate sweep)
                     if (sd < 1.0e38) seed_d = sd, seed2 = sd * sd * (1.0 + 1e-6);
                 }
                 const double qx = s_ps.R[0] * px + s_ps.R[1] * py + s_ps.R[2] * pz + s_ps.t[0];
@@ -1017,7 +1047,8 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
             const unsigned left = atomicAdd(&st->exit_ctr, 1u);
             if (left == gridDim.x - 1) {
                 st->win_ctr = 0, st->arrive = 0, st->abort = 0, st->a_arrive = 0;
-                for (int k = 0; k < KICP_MAX_ITERATIONS; ++k) st->todo_n[k] = 0, st->slow_n[k] = 0;
+                for (int c = 0; c < KR_CLASSES; ++c)
+                    for (int k = 0; k < KICP_MAX_ITERATIONS; ++k) st->cls_n[c][k] = 0;
                 __threadfence();
                 st->exit_ctr = 0;
             }

@@ -50,9 +50,14 @@ struct KernelArgs {
     // nearest-neighbour cache carried from pass to pass (persistent kernel, option "nn_cache"), one entry per scan point
     unsigned int *nn_g;            // the neighbour found by the last search (global point index, 0xFFFFFFFF = none)
     unsigned int *nn_g2;           // the runner-up of that search (0xFFFFFFFF = none): between passes the two may swap
-    float *nn_l;                   // certified lower bound on the distance to every candidate OTHER than those two
-    float *nn_seed;                // distance to the old neighbour from the new position (pruning bound of the repeated search)
-    unsigned int *todo;            // points of the current pass that need the search
+    float *nn_l;                   // certified lower bound on the distance to every candidate OTHER than those two; for a point that is
+                                   // searched again, from the certificate sweep to its search: the distance to the old neighbour from
+                                   // the new position (the pruning bound of that search)
+    unsigned int *todo;            // points of the current pass that need the search: two cost classes, one from each end ...
+    union {
+        unsigned int *todo2;       // ... and the other two (same size)
+        float *nn_seed;            // (the name the CPU test harness in tests/emu gives this buffer)
+    };
     kicp_reg_result *result_host;   // optional: device-visible alias of the caller's page-locked result block (written by CTA 0 at the end)
     unsigned long long timeout_ns;  // device-side waits (upload flags, peers) give up after this long
 };

@@ -139,7 +139,7 @@ static int enqueue_registration(kicp_map *m, const kicp_scan *scan, const double
         ka.pow2_voxel = std::frexp(m->voxel_size, &e) == 0.5 ? 1 : 0;
     }
     ka.collect_stats = c->collect_stats;
-    ka.nn_g = nullptr, ka.nn_g2 = nullptr, ka.nn_l = nullptr, ka.nn_seed = nullptr, ka.todo = nullptr;
+    ka.nn_g = nullptr, ka.nn_g2 = nullptr, ka.nn_l = nullptr, ka.todo = nullptr, ka.todo2 = nullptr;
     // (1 = automatic: a small scan is one tiny window per warp and gains nothing from the extra phase and its barrier)
     // a frame whose exact count is still on the device is planned (grid, certificates) for the count its producer expects
     const int64_t n_plan = (scan->d_n && c->reg_n_hint > 0) ? std::min<int64_t>(c->reg_n_hint, scan->n) : scan->n;
@@ -147,17 +147,17 @@ static int enqueue_registration(kicp_map *m, const kicp_scan *scan, const double
     if ((c->nn_cache == 2 || (c->nn_cache == 1 && n_plan >= 49152)) && scan->n > 0) {
         if (scan->n > c->nn_cap) {
             KICP_CUDA(cudaStreamSynchronize(c->stream));
-            cudaFree(c->d_nn_g), cudaFree(c->d_nn_g2), cudaFree(c->d_nn_l), cudaFree(c->d_nn_seed), cudaFree(c->d_todo);
-            c->d_nn_g = nullptr, c->d_nn_g2 = nullptr, c->d_nn_l = nullptr, c->d_nn_seed = nullptr, c->d_todo = nullptr, c->nn_cap = 0;
+            cudaFree(c->d_nn_g), cudaFree(c->d_nn_g2), cudaFree(c->d_nn_l), cudaFree(c->d_todo), cudaFree(c->d_todo2);
+            c->d_nn_g = nullptr, c->d_nn_g2 = nullptr, c->d_nn_l = nullptr, c->d_todo = nullptr, c->d_todo2 = nullptr, c->nn_cap = 0;
             const int64_t cap = scan->n + scan->n / 4 + 1024;
             KICP_CUDA(cudaMalloc(&c->d_nn_g, (size_t)cap * sizeof(unsigned int)));
             KICP_CUDA(cudaMalloc(&c->d_nn_g2, (size_t)cap * sizeof(unsigned int)));
             KICP_CUDA(cudaMalloc(&c->d_nn_l, (size_t)cap * sizeof(float)));
-            KICP_CUDA(cudaMalloc(&c->d_nn_seed, (size_t)cap * sizeof(float)));
             KICP_CUDA(cudaMalloc(&c->d_todo, (size_t)cap * sizeof(unsigned int)));
+            KICP_CUDA(cudaMalloc(&c->d_todo2, (size_t)cap * sizeof(unsigned int)));
             c->nn_cap = cap;
         }
-        ka.nn_g = c->d_nn_g, ka.nn_g2 = c->d_nn_g2, ka.nn_l = c->d_nn_l, ka.nn_seed = c->d_nn_seed, ka.todo = c->d_todo;
+        ka.nn_g = c->d_nn_g, ka.nn_g2 = c->d_nn_g2, ka.nn_l = c->d_nn_l, ka.todo = c->d_todo, ka.todo2 = c->d_todo2;
     }
     ka.timeout_ns = (unsigned long long)c->spin_timeout_ms * 1000000ull;
     // A result block in page-locked host memory (kicp_host_alloc, the context's own staging) is written by the persistent kernel
