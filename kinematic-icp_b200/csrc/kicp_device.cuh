@@ -111,6 +111,22 @@ __device__ __forceinline__ void quat_rotate(double qx, double qy, double qz, dou
     oy = py + qw * uy + (qz * ux - qx * uz);
     oz = pz + qw * uz + (qx * uy - qy * ux);
 }
+// a + b with one rounding of the exact sum, never contracted with a neighbouring product: an FMA with a unit factor is exactly
+// that (and, unlike __dadd_rn, it is among the intrinsics the host-side kernel emulator of tests/emu supplies)
+__device__ __forceinline__ double add_rn(double a, double b) { return __fma_rn(a, 1.0, b); }
+
+// The same rotation with every operation rounded on its own (__dmul_rn / add_rn): the reference's plain IEEE result bit for bit
+// in a file that is compiled with FMA contraction (kicp_register.cu).
+__device__ __forceinline__ void quat_rotate_rn(double qx, double qy, double qz, double qw, double px, double py, double pz,
+                                               double &ox, double &oy, double &oz) {
+    double ux = add_rn(__dmul_rn(qy, pz), -__dmul_rn(qz, py));
+    double uy = add_rn(__dmul_rn(qz, px), -__dmul_rn(qx, pz));
+    double uz = add_rn(__dmul_rn(qx, py), -__dmul_rn(qy, px));
+    ux = add_rn(ux, ux), uy = add_rn(uy, uy), uz = add_rn(uz, uz);
+    ox = add_rn(add_rn(px, __dmul_rn(qw, ux)), add_rn(__dmul_rn(qy, uz), -__dmul_rn(qz, uy)));
+    oy = add_rn(add_rn(py, __dmul_rn(qw, uy)), add_rn(__dmul_rn(qz, ux), -__dmul_rn(qx, uz)));
+    oz = add_rn(add_rn(pz, __dmul_rn(qw, uz)), add_rn(__dmul_rn(qx, uy), -__dmul_rn(qy, ux)));
+}
 __device__ __forceinline__ void pose_apply(const Pose &T, double px, double py, double pz, double &ox, double &oy, double &oz) {
     quat_rotate(T.qx, T.qy, T.qz, T.qw, px, py, pz, ox, oy, oz);
     ox += T.tx, oy += T.ty, oz += T.tz;

@@ -208,19 +208,31 @@ struct __align__(16) WarpSm {
     unsigned short task[KR_TCAP];    // task stream of the current stage: owner << 5 | shift index
 };
 
-// The reference compares NORMS with a strict < (first minimum wins).  sqrt is monotone, so the squares decide — except when two
-// squares within an ulp or two round to the same norm: then the earlier point stays.  Kept out of line: it is needed about never.
+// The reference compares NORMS with a strict < (first minimum wins).  d2 and best are the reference's own squares (dist2 at the
+// reference's query, query_rn); sqrt is monotone, so the squares decide — except when two squares within an ulp or two round to the
+// same norm: then the earlier point stays.  So the association of the first pass is the reference's, point for point, given the
+// same prior (later passes start from a pose whose last bits depend on the summation order).  Kept out of line: needed about never.
 __device__ __noinline__ bool same_norm(double a, double b) { return sqrt(a) == sqrt(b); }
-__device__ __forceinline__ bool closer(double d2, double best) {  // "norm(d2) < norm(best)" as the reference would evaluate it
+__device__ __forceinline__ bool closer(double d2, double best) {  // "norm(d2) < norm(best)" as the reference evaluates it
     if (!(d2 < best)) return false;
     if (d2 >= best * (1.0 - 4e-16)) return !same_norm(d2, best);
     return true;
 }
 
-// |c - q|^2 with a pinned operation order (the owner re-evaluates the winning line: both evaluations must agree bit for bit)
+// |c - q|^2 as the reference's (c - q).norm() squares it: (dx dx + dy dy) + dz dz, every operation rounded on its own (an FMA
+// would give other squares, and two points the reference sees at the same distance could then differ here).  The owner
+// re-evaluates the winning line with it: both evaluations agree bit for bit.
 __device__ __forceinline__ double dist2(double cx, double cy, double cz, double qx, double qy, double qz) {
     const double dx = cx - qx, dy = cy - qy, dz = cz - qz;
-    return __fma_rn(dz, dz, __fma_rn(dy, dy, __dmul_rn(dx, dx)));
+    return add_rn(add_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+}
+
+// q = T p as the reference evaluates it: Sophus' quaternion rotation, then the translation (Registration.cpp:74), without FMA
+// contraction — the query of the search is the reference's to the last bit (the rotation matrix R would differ in the last bits)
+__device__ __forceinline__ void query_rn(const double q[4], const double t[3], double px, double py, double pz, double &ox, double &oy,
+                                         double &oz) {
+    quat_rotate_rn(q[0], q[1], q[2], q[3], px, py, pz, ox, oy, oz);
+    ox = add_rn(ox, t[0]), oy = add_rn(oy, t[1]), oz = add_rn(oz, t[2]);
 }
 
 __device__ __forceinline__ void load_scan_point(const ScanView &sv, int i, double &x, double &y, double &z) {
@@ -405,12 +417,11 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                 const bool haveg = g1 != 0xFFFFFFFFu, have2 = g2 != 0xFFFFFFFFu;
                 const Point4 c1 = ld_point(a.map.pts + (size_t)(haveg ? g1 : 0u) * KICP_PSTRIDE);
                 const Point4 c2 = ld_point(a.map.pts + (size_t)(have2 ? g2 : 0u) * KICP_PSTRIDE);
-                const double qx = s_ps.R[0] * px + s_ps.R[1] * py + s_ps.R[2] * pz + s_ps.t[0];
-                const double qy = s_ps.R[3] * px + s_ps.R[4] * py + s_ps.R[5] * pz + s_ps.t[1];
-                const double qz = s_ps.R[6] * px + s_ps.R[7] * py + s_ps.R[8] * pz + s_ps.t[2];
-                const double ox = s_ps.Rp[0] * px + s_ps.Rp[1] * py + s_ps.Rp[2] * pz + s_ps.tp[0];
-                const double oy = s_ps.Rp[3] * px + s_ps.Rp[4] * py + s_ps.Rp[5] * pz + s_ps.tp[1];
-                const double oz = s_ps.Rp[6] * px + s_ps.Rp[7] * py + s_ps.Rp[8] * pz + s_ps.tp[2];
+                // the query of this pass and the previous one, both as the search evaluates them (query_rn): the search of this
+                // pass starts from the very q the certificate was judged at, and o is bit for bit the query the previous search used
+                double qx, qy, qz, ox, oy, oz;
+                query_rn(s_ps.q, s_ps.t, px, py, pz, qx, qy, qz);
+                query_rn(s_ps.qp, s_ps.tp, px, py, pz, ox, oy, oz);
                 const double vs = a.map.voxel_size;
                 const int vx = voxel_of(qx, vs, inv_vs, a.pow2_voxel), vy = voxel_of(qy, vs, inv_vs, a.pow2_voxel),
                           vz = voxel_of(qz, vs, inv_vs, a.pow2_voxel);
@@ -602,9 +613,8 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                     const double sd = (double)__ldcg(&a.nn_l[pi]);  // (the seed, left there by the certificate sweep)
                     if (sd < 1.0e38) seed_d = sd, seed2 = sd * sd * (1.0 + 1e-6);
                 }
-                const double qx = s_ps.R[0] * px + s_ps.R[1] * py + s_ps.R[2] * pz + s_ps.t[0];
-                const double qy = s_ps.R[3] * px + s_ps.R[4] * py + s_ps.R[5] * pz + s_ps.t[1];
-                const double qz = s_ps.R[6] * px + s_ps.R[7] * py + s_ps.R[8] * pz + s_ps.t[2];
+                double qx, qy, qz;
+                query_rn(s_ps.q, s_ps.t, px, py, pz, qx, qy, qz);
                 sm.qxy[lane] = make_double2(qx, qy), sm.qz[lane] = qz;
                 sm.vx[lane] = voxel_of(qx, a.map.voxel_size, inv_vs, a.pow2_voxel);
                 sm.vy[lane] = voxel_of(qy, a.map.voxel_size, inv_vs, a.pow2_voxel);

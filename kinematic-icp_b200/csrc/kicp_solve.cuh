@@ -15,7 +15,7 @@ struct PoseState {
     double q[4];  // current estimate: unit quaternion (x, y, z, w) ...
     double t[3];  // ... translation ...
     double R[9];  // ... and the rotation matrix of q, row-major
-    double Rp[9], tp[3];  // R, t of the previous pass (the nearest-neighbour certificates compare the two)
+    double qp[4], tp[3];  // q, t of the previous pass (the nearest-neighbour certificates compare the two)
     double tau, conv, fixed_reg, beta;
     int adaptive, max_iter;
     int iter, done, status;
@@ -97,9 +97,9 @@ __device__ void pose_init(PoseState *ps, const RegArgs &a) {
     double q[4], t[3], R[9];
     se3_compose(lq, lt, oq, ot, q, t);
     quat_to_matrix(q, R);
-    for (int k = 0; k < 4; ++k) ps->q[k] = q[k];
+    for (int k = 0; k < 4; ++k) ps->q[k] = q[k], ps->qp[k] = q[k];
     for (int k = 0; k < 3; ++k) ps->t[k] = t[k];
-    for (int k = 0; k < 9; ++k) ps->R[k] = R[k], ps->Rp[k] = R[k];
+    for (int k = 0; k < 9; ++k) ps->R[k] = R[k];
     for (int k = 0; k < 3; ++k) ps->tp[k] = t[k];
     ps->tau = a.tau, ps->conv = a.conv, ps->fixed_reg = a.fixed_reg, ps->beta = 0.0;
     ps->adaptive = a.adaptive, ps->max_iter = a.max_iter;
@@ -141,7 +141,7 @@ __device__ void solve_and_update(PoseState *ps, const double *s, kicp_reg_result
     se3_exp_planar(ux, uy, dx1, dq, dt);
     se3_compose(cq, ct, dq, dt, nq, nt);  // current_estimate = current_estimate * delta_motion  (:182)
     quat_to_matrix(nq, nR);
-    for (int k = 0; k < 9; ++k) ps->Rp[k] = ps->R[k];
+    for (int k = 0; k < 4; ++k) ps->qp[k] = ps->q[k];
     for (int k = 0; k < 3; ++k) ps->tp[k] = ps->t[k];
     for (int k = 0; k < 4; ++k) ps->q[k] = nq[k];
     for (int k = 0; k < 3; ++k) ps->t[k] = nt[k];

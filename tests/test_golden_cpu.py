@@ -4,6 +4,8 @@ import os
 import numpy as np
 import pytest
 
+from scenes import fuzz_cases
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
@@ -62,35 +64,6 @@ def test_pipeline_golden_is_reproducible(oracle):
     poses, n_src, n_map = S.run_pipeline(pipe, seq)
     pipe.close()
     assert np.array_equal(poses, z["deskew_poses"]) and np.array_equal(n_map, z["deskew_n_map"])
-
-
-def fuzz_cases(ko):
-    """40 small random scenes and random solver settings (0..25 iterations, adaptive / fixed regularisation, gates from 5 cm to
-    3 m, empty scans), each as (oracle map, its voxel-grouped points, scan, last pose, odometry, tau, solver settings)."""
-    from oracle.workloads import unicycle
-    rng = np.random.default_rng(20260923)
-    for case in range(40):
-        vs = float(rng.choice([0.5, 1.0, 2.0]))
-        cap = int(rng.choice([1, 5, 20]))
-        # a bumpy ground patch plus two walls, mapped from a few random poses
-        n_map = int(rng.integers(500, 6000))
-        ground = np.c_[rng.uniform(-25, 25, (n_map, 2)), 0.05 * rng.standard_normal(n_map)]
-        wall = np.c_[rng.uniform(-25, 25, n_map // 2), np.full(n_map // 2, 12.0) + 0.02 * rng.standard_normal(n_map // 2),
-                     rng.uniform(0, 4, n_map // 2)]
-        om = ko.OracleMap(vs, 100.0, cap)
-        pts = np.concatenate([ground, wall])
-        om.add_points(pts)
-        _, _, stored = om.export_voxels()
-        last = ko.planar_pose(*rng.uniform(-3, 3, 2), rng.uniform(-3.1, 3.1))
-        true_rel = unicycle(rng.uniform(0.0, 1.0), rng.uniform(-0.1, 0.1))
-        odom = unicycle(rng.uniform(0.0, 1.1), rng.uniform(-0.12, 0.12))
-        n_scan = int(rng.integers(0, 3000))
-        world = pts[rng.integers(0, len(pts), n_scan)] + 0.01 * rng.standard_normal((n_scan, 3))
-        scan = ko.se3_transform(ko.se3_inverse(ko.se3_compose(last, true_rel)), world) if n_scan else np.zeros((0, 3))
-        tau = float(rng.choice([0.05, 0.3, 1.0, 3.0]))
-        kw = dict(max_iter=int(rng.choice([0, 1, 3, 10, 25])), conv=float(rng.choice([1e-3, 1e-6, 1e-1])),
-                  adaptive=bool(rng.integers(0, 2)), fixed_reg=float(rng.choice([0.0, 0.1, 10.0])))
-        yield om, vs, cap, stored, scan, last, odom, tau, kw
 
 
 def test_oracle_matches_reference_build_fuzz(oracle):

@@ -22,6 +22,7 @@ TOL_T, TOL_R = 1e-6, 1e-7
 
 
 from emu import harness as H
+import scenes as S
 
 
 @pytest.fixture(scope="module")
@@ -153,3 +154,71 @@ def test_kernel_vs_reference_golden(emu, oracle, name):
                      adaptive=bool(case[2]), fixed_reg=case[3])
         dt, ang = ko.pose_delta(r.pose_np(), case[5:])
         assert dt <= TOL_T and ang <= TOL_R, (dt, ang)
+
+
+# ------------------------------------------------------------------------------------------ ties, map shapes, randomised scenes
+TIE_IDS = ["permuted-vs1", "permuted-vs0.5", "permuted-rotated", "stage-vs1", "stage-vs0.5", "near-vs1", "near-vs0.5", "near-rotated"]
+SHAPE_IDS = ["vs0.3-cap1", "vs0.75-cap24", "vs0.6-cap25", "vs0.75-cap29-far", "vs0.3-cap255", "vs0.75-cap20-utm"]
+LAUNCHES = [(1, 1, 0), (2, 1, 1), (3, 0, 0)]  # (grid, persistent, certificates)
+
+
+@pytest.fixture(scope="module")
+def tie_scenes(oracle):
+    return S.tie_scenes(oracle)
+
+
+@pytest.fixture(scope="module")
+def shape_scenes(oracle):
+    return S.shape_scenes(oracle)
+
+
+@pytest.mark.parametrize("k", range(len(TIE_IDS)), ids=TIE_IDS)
+def test_neighbour_ties_match_reference(emu, oracle, tie_scenes, k):
+    """Exact ties and ulp-level near-ties of the first pass: the kernel must take the reference's point at every query (exact N,
+    sums to 1e-9, the pose).  Each permuted-tie scene holds pairs at which squaring with an FMA picks the other point."""
+    sc = tie_scenes[k]
+    if TIE_IDS[k].startswith("permuted"):
+        assert sc.traps >= 5, sc.traps
+    for grid, persistent, cache in LAUNCHES:
+        check(emu, oracle, sc.om, sc.scan, sc.last, sc.odom, sc.tau, grid=grid, persistent=persistent, nn_cache=cache, **sc.kw)
+
+
+def test_map_kernel_nearest_on_ties(oracle, tie_scenes):
+    """The map kernels' batched GetClosestNeighbor (built without FMA contraction) on the same ties: point and distance bit for bit."""
+    for sc in tie_scenes:
+        em = H.EmuMap(sc.voxel_size, S.FAR, sc.cap)
+        try:
+            em.load_voxels(*sc.voxels)
+            q = sc.queries(oracle)
+            pe, de = em.nearest(q)
+            po, do = sc.om.nearest(q)
+            assert np.array_equal(de, do) and np.array_equal(pe, po), sc.name
+        finally:
+            em.close()
+
+
+@pytest.mark.parametrize("k", range(len(SHAPE_IDS)), ids=SHAPE_IDS)
+def test_map_shapes_match_oracle(emu, oracle, shape_scenes, k):
+    """Voxel sizes that are not powers of two (the division branch of voxel_of), voxels filled to caps of 1 to 255 (fewer than 32
+    tasks per batch, a full line buffer), queries exactly on voxel faces and at negative coordinates, maps far from the origin."""
+    sc = shape_scenes[k]
+    assert np.frexp(sc.voxel_size)[0] != 0.5 and np.all(sc.voxels[1] == sc.cap)
+    for grid, persistent, cache in LAUNCHES:
+        check(emu, oracle, sc.om, sc.scan, sc.last, sc.odom, sc.tau, grid=grid, persistent=persistent, nn_cache=cache, **sc.kw)
+
+
+def test_fuzz_scenes_vs_reference(emu, oracle):
+    """The 40 randomised scenes of the oracle's pin (voxel 0.5 / 1 / 2, caps 1 / 5 / 20, gates from 5 cm to 3 m, 0 to 25
+    iterations, empty scans) through the kernel, against the poses the reference's own sources returned: same NaN pattern, pose
+    within the north-star tolerance.  Launch shapes and certificates alternate from scene to scene."""
+    ref = np.load(os.path.join(GOLDEN, "ref_fuzz.npz"))["poses"]
+    ran = 0
+    for case, (om, _, _, _, scan, last, odom, tau, kw) in enumerate(S.fuzz_cases(oracle)):
+        res, _ = run_emu(emu, om, scan, last, odom, tau, grid=1 + case % 3, nn_cache=case % 2, **kw)
+        pose, pr = res[0].pose_np(), ref[case]
+        assert np.array_equal(np.isnan(pose), np.isnan(pr)), (case, kw)
+        if not np.isnan(pr).any():
+            dt, ang = oracle.pose_delta(pose, pr)
+            assert dt <= TOL_T and ang <= TOL_R, (case, kw, dt, ang)
+        ran += 1
+    assert case == 39 and ran == 40
