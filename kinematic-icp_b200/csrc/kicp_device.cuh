@@ -1,6 +1,7 @@
 // Device-side helpers shared by the map and registration kernels.
 #pragma once
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <math.h>
 #include <stdint.h>
 
@@ -48,9 +49,23 @@ __host__ __device__ __forceinline__ uint32_t voxel_hash(int x, int y, int z) {
     return h;
 }
 
+// static_cast<int>(floor(q)) as the reference's x86-64 build evaluates it (cvttsd2si): NaN, +-Inf and anything whose floor is
+// outside [-2^31, 2^31) become INT_MIN.  A plain (int) cast compiles to cvt.rzi.s32.f64 on the device, which gives 0 for NaN and
+// saturates to INT_MAX above, so a non-finite or huge point would land in another voxel than the reference's.  On the device
+// cvt.rmi.s32.f64 (__double2int_rd) floors and saturates below to INT_MIN already, so one comparison (false for NaN) fixes up NaN and
+// the values above; the host form (the CPU emulator of tests/emu) spells the rule out.
+__host__ __device__ __forceinline__ int voxel_floor(double q) {
+#ifdef __CUDA_ARCH__
+    return q < 2147483648.0 ? __double2int_rd(q) : INT_MIN;
+#else
+    const double f = floor(q);
+    return f >= -2147483648.0 && f < 2147483648.0 ? (int)f : INT_MIN;
+#endif
+}
+
 // PointToVoxel (KISS VoxelUtils.hpp): static_cast<int>(floor(x / voxel_size)).  A true FP64 division, not a
 // multiplication by the reciprocal, so voxel boundaries fall exactly where the reference puts them.
-__device__ __forceinline__ int voxel_coord(double x, double vs) { return (int)floor(x / vs); }
+__device__ __forceinline__ int voxel_coord(double x, double vs) { return voxel_floor(x / vs); }
 
 // DIVERGENCE SAFETY.  nvcc keeps loop-invariant kernel parameters (table mask, base pointers) in UNIFORM registers,
 // which are shared by the 32 lanes of a warp.  Inside a per-lane loop (a hash-probe chain, a voxel scan) that is only

@@ -287,6 +287,9 @@ __global__ void k_nearest(MapView m, const double *__restrict__ q, int64_t n, do
         for (int j = 0; j < cnt; ++j) {
             const double dx = vp[KICP_PSTRIDE * j] - qx, dy = vp[KICP_PSTRIDE * j + 1] - qy, dz = vp[KICP_PSTRIDE * j + 2] - qz;
             const double d = sqrt(dx * dx + dy * dy + dz * dz);
+            // the reference takes a voxel's min_element first: a NaN distance of its FIRST point (a non-finite point in the map or
+            // the query) is never replaced and never wins, so the whole voxel drops out; a later NaN is skipped by the strict <
+            if (j == 0 && d != d) break;
             if (d < bd) bd = d, bx = vp[KICP_PSTRIDE * j], by = vp[KICP_PSTRIDE * j + 1], bz = vp[KICP_PSTRIDE * j + 2];
         }
     }

@@ -330,8 +330,9 @@ __device__ __forceinline__ void accumulate(WarpSm &sm, int lane, const PoseState
 
 __device__ __forceinline__ int voxel_of(double x, double vs, double inv_vs, int pow2) {
     // PointToVoxel: floor(x / voxel_size); for a power-of-two voxel size the product with the (exact) reciprocal is the same
-    // double as the quotient, so the cheaper form is used
-    return pow2 ? (int)floor(x * inv_vs) : voxel_coord(x, vs);
+    // double as the quotient, so the cheaper form is used; both convert like voxel_coord, or the keys the map stores and the keys
+    // probed here would disagree for non-finite and huge coordinates
+    return pow2 ? voxel_floor(x * inv_vs) : voxel_coord(x, vs);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

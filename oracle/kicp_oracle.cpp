@@ -168,11 +168,13 @@ void se3_log(const SE3 &T, double out[6]) {
 }
 
 // ------------------------------------------------------------------ KISS-ICP v1.2.0 map
-// VoxelUtils.hpp PointToVoxel: floor, not truncation
-Voxel PointToVoxel(const Vec3 &p, double vs) {
-    return {static_cast<int32_t>(std::floor(p.x / vs)), static_cast<int32_t>(std::floor(p.y / vs)),
-            static_cast<int32_t>(std::floor(p.z / vs))};
+// VoxelUtils.hpp PointToVoxel: floor, not truncation.  static_cast<int> of a NaN, an infinity or a value outside the int range is
+// undefined behaviour in C++; the reference's x86-64 build (cvttsd2si) gives INT_MIN for all of them, spelled out here.
+static int32_t floor_to_voxel(double q) {
+    const double f = std::floor(q);
+    return f >= -2147483648.0 && f < 2147483648.0 ? static_cast<int32_t>(f) : INT32_MIN;
 }
+Voxel PointToVoxel(const Vec3 &p, double vs) { return {floor_to_voxel(p.x / vs), floor_to_voxel(p.y / vs), floor_to_voxel(p.z / vs)}; }
 
 // VoxelHashMap.cpp voxel_shifts: centre, 6 faces, 12 edges, 8 corners
 const Voxel kVoxelShifts[27] = {

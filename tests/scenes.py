@@ -353,3 +353,247 @@ def fuzz_cases(ko):
         kw = dict(max_iter=int(rng.choice([0, 1, 3, 10, 25])), conv=float(rng.choice([1e-3, 1e-6, 1e-1])),
                   adaptive=bool(rng.integers(0, 2)), fixed_reg=float(rng.choice([0.0, 0.1, 10.0])))
         yield om, vs, cap, stored, scan, last, odom, tau, kw
+
+
+# --------------------------------------------------------------------------------------------------------------- edges
+# Scenes that sit on the decisions of the map and front-end kernels: points on voxel faces, norms equal to the range gate,
+# candidates exactly map_resolution from a stored point, first points exactly max_distance from the origin, probe chains that
+# wrap past the last slot of the table, and coordinates that are not finite or do not fit an int once divided by the voxel size.
+NAN, INF = float("nan"), float("inf")
+
+
+def bits(a):
+    """The bit patterns of a float64 array: equal arrays compare equal, NaN included."""
+    return np.ascontiguousarray(a, dtype=np.float64).view(np.uint64)
+
+
+def same_bits(a, b):
+    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
+    return a.shape == b.shape and np.array_equal(bits(a), bits(b))
+
+
+def floor_key(x, vs):
+    """PointToVoxel of one coordinate as the reference's x86-64 build evaluates it: NaN, +-Inf and values outside the int range
+    become INT_MIN."""
+    f = math.floor(x / vs) if math.isfinite(x / vs) else None
+    return f if f is not None and -2 ** 31 <= f < 2 ** 31 else -2 ** 31
+
+
+def boundary_cloud(vs, origin=0.0, span=6):
+    """Points at exact multiples k vs of the voxel size (k in [-span, span]) and one ulp either side of them, on every axis and
+    on both signs, +0.0 and -0.0, around a scalar `origin` (UTM-like offsets: 5e5, 4e6).  Returns the cloud, how many of its
+    coordinates a reciprocal multiply x * (1 / vs) puts in another voxel than x / vs, and how many have a quotient that rounds up
+    onto an integer that the exact quotient does not reach."""
+    xs = []
+    base = math.floor(origin / vs)
+    for k in range(base - span, base + span + 1):
+        x = k * vs
+        xs += [x, np.nextafter(x, -INF), np.nextafter(x, INF)]
+        # the doubles just below k vs whose quotient still rounds onto k: exact arithmetic would floor them to k - 1
+        y = np.nextafter(x, -INF)
+        for _ in range(4):
+            y = np.nextafter(y, -INF)
+            xs.append(y)
+    xs += [0.0, -0.0]
+    # and, from further out, the doubles next to multiples of vs where x * (1 / vs) floors into another voxel than x / vs
+    inv = 1.0 / vs
+    ks = np.arange(base - 4000, base + 4001, dtype=np.float64) * vs
+    for steps in range(-3, 4):
+        c = ks
+        for _ in range(abs(steps)):
+            c = np.nextafter(c, INF if steps > 0 else -INF)
+        xs += list(c[np.floor(c / vs) != np.floor(c * inv)][:6])
+    xs = np.array(xs)
+    flips = int(sum(math.floor(x / vs) != math.floor(x * inv) for x in xs))
+    rounded = int(sum(math.floor(x / vs) != math.floor(Fraction(x) / Fraction(vs)) for x in xs))
+    n = len(xs)
+    rng = np.random.default_rng(int(vs * 1000) + int(origin) % 1000)
+    pts = []
+    for ax in range(3):  # one coordinate on the boundary, the others anywhere in a voxel near it (also on boundaries)
+        p = np.empty((n, 3))
+        p[:, ax] = xs
+        for o in range(3):
+            if o != ax:
+                p[:, o] = xs[rng.permutation(n)] if o == (ax + 1) % 3 else origin + rng.uniform(-3, 3, n) * vs
+        pts.append(p)
+    pts.append(np.stack([xs, xs[::-1], xs[rng.permutation(n)]], 1))
+    return np.concatenate(pts), flips, rounded
+
+
+def boundary_clouds():
+    """(cloud, voxel size, reciprocal flips, rounded-up quotients): voxel sizes that are not powers of two (0.37, 0.3, 0.1) and
+    the pipeline's own 0.5 vs and 1.5 vs of a 1.0 map, near the origin and at UTM-like offsets."""
+    return [(vs,) + boundary_cloud(vs, origin) for vs in (0.37, 0.3, 0.1, 0.5, 1.5) for origin in (0.0, 5e5, 4e6)]
+
+
+def range_gate_cloud(min_range, max_range):
+    """Points whose norm sqrt(x x + y y + z z) is exactly min_range or max_range (axis points and (3, 4, 12) 2^k, norm 13 2^k), one
+    ulp inside and outside, and the zero point.  Both ranges must be 13 2^k.  Returns the cloud and the norms the reference sees."""
+    pts = []
+    for r in (min_range, max_range):
+        m, e = math.frexp(r / 13.0)
+        assert m == 0.5, "ranges of the form 13 2^k"
+        for sgn in (1.0, -1.0):
+            for ax in range(3):
+                p = np.zeros(3)
+                p[ax] = sgn * r
+                pts += [p.copy()]
+                for d in (-INF, INF):
+                    q = p.copy()
+                    q[ax] = np.nextafter(p[ax], d)
+                    pts.append(q)
+            t = np.array([3.0, 4.0, 12.0]) * (r / 13.0) * sgn
+            pts.append(t)
+            for ax in range(3):
+                for d in (-INF, INF):
+                    q = t.copy()
+                    q[ax] = np.nextafter(t[ax], d)
+                    pts.append(q)
+    pts.append(np.zeros(3))
+    pts.append(np.array([-0.0, 0.0, -0.0]))
+    pts = np.array(pts)
+    norms = np.sqrt(pts[:, 0] * pts[:, 0] + pts[:, 1] * pts[:, 1] + pts[:, 2] * pts[:, 2])
+    return pts, norms
+
+
+def map_rule_points(vs=1.0, cap=4, n_voxels=24, seed=11):
+    """Points for AddPoints whose candidates sit exactly map_resolution = sqrt(vs^2 / cap) from a stored point (kept: the rule is
+    a strict <) or one ulp closer (dropped), along each axis, in voxels on both sides of the origin.  vs and cap are chosen so
+    that map_resolution is exact (vs 1: cap 4 gives 0.5, cap 16 gives 0.25).  Returns the points and (exact, one ulp closer)
+    counts of candidates, measured against the first point of their voxel."""
+    res = math.sqrt(vs * vs / cap)
+    assert res * res == vs * vs / cap
+    rng = np.random.default_rng(seed)
+    pts, exact, closer = [], 0, 0
+    for i in range(n_voxels):
+        v = (_lattice(i, spacing=2, side=4) * vs).astype(np.float64)
+        a = v + _dyadic(rng.uniform(0.05, 0.4, 3) * vs, 2.0 ** -12)
+        pts.append(a)
+        ax = i % 3
+        b = a.copy()
+        b[ax] = a[ax] + res
+        if i % 2:
+            b[ax] = np.nextafter(b[ax], a[ax])  # one ulp closer
+        dx = b[ax] - a[ax]
+        dist = math.sqrt(dx * dx)
+        if i % 2 == 0:
+            assert dist == res
+            exact += 1
+        else:
+            assert dist < res
+            closer += 1
+        assert floor_key(b[ax], vs) == floor_key(a[ax], vs)
+        pts.append(b)
+        for _ in range(cap + 2):  # more than the cap: the voxel fills up and the rest is skipped
+            pts.append(v + _dyadic(rng.uniform(0.0, 1.0, 3) * vs, 2.0 ** -12))
+    return np.array(pts), exact, closer
+
+
+def far_first_points(max_distance=12.0, vs=3.0):
+    """First points of voxels exactly max_distance from the origin (dx^2 + dy^2 + dz^2 == max_distance^2 exactly: evicted by
+    the >= rule), one ulp inside (kept), and voxels whose far first point is followed by near later points (the first point
+    decides).  Returns the points and the squared norms of the first points."""
+    md = max_distance
+    firsts = [np.array([md, 0, 0]), np.array([0, -md, 0]), np.array([0, 0, md]),
+              np.array([np.nextafter(md, 0.0), 0, 0]), np.array([0, np.nextafter(-md, 0.0), 0]),
+              np.array([md * 0.6, md * 0.8, 0.0]) if (md * 0.6) ** 2 + (md * 0.8) ** 2 == md * md else np.array([0, 0, -md])]
+    pts = []
+    for f in firsts:
+        pts.append(f)
+        v = np.floor(f / vs) * vs
+        pts.append(v + 0.25 * vs)  # a later point of the same voxel, nearer the origin
+    # a far first point (outside max_distance) followed by near points of the same voxel
+    f = np.array([3.9 * vs, 3.9 * vs, 0.1])
+    assert float(f @ f) >= md * md
+    pts += [f, np.array([3.05 * vs, 3.05 * vs, 0.1]), np.array([3.1 * vs, 3.2 * vs, 0.2])]
+    pts = np.array(pts, dtype=np.float64)
+    sq = np.array([x[0] * x[0] + x[1] * x[1] + x[2] * x[2] for x in firsts])
+    return pts, sq
+
+
+def voxel_hash_np(x, y, z):
+    """voxel_hash of kicp_device.cuh (the reference's three-prime XOR, then a murmur3 finaliser) on integer arrays."""
+    u = lambda a: np.asarray(a, dtype=np.int64).astype(np.uint32)
+    with np.errstate(over="ignore"):
+        h = (u(x) * np.uint32(73856093)) ^ (u(y) * np.uint32(19349669)) ^ (u(z) * np.uint32(83492791))
+        h ^= h >> np.uint32(16)
+        h *= np.uint32(0x85EBCA6B)
+        h ^= h >> np.uint32(13)
+        h *= np.uint32(0xC2B2AE35)
+        h ^= h >> np.uint32(16)
+    return h
+
+
+_COLLIDING = {}
+
+
+def colliding_keys(bits=18, half=128):
+    """Voxel keys of the cube [-half, half)^3 whose hash has its low `bits` bits all set: they share the LAST home slot of every
+    table of up to 2^bits slots, so a chain of them wraps past slot 0 whatever the table's size."""
+    if (bits, half) not in _COLLIDING:
+        r = np.arange(-half, half, dtype=np.int64)
+        Y, Z = np.meshgrid(r, r, indexing="ij")
+        Y, Z = Y.ravel(), Z.ravel()
+        want = np.uint32((1 << bits) - 1)
+        found = []
+        for x in r:
+            h = voxel_hash_np(np.full_like(Y, x), Y, Z)
+            sel = np.flatnonzero((h & want) == want)
+            found += [(int(x), int(Y[i]), int(Z[i])) for i in sel]
+        _COLLIDING[(bits, half)] = np.array(found, dtype=np.int64)
+    return _COLLIDING[(bits, half)]
+
+
+def collision_scene(ko, n_map, vs=1.0, cap=5, n_absent=6, seed=13, max_distance=FAR):
+    """A map of `n_map` voxels whose keys all collide (one chain that starts at the last slot and wraps), each holding `cap`
+    points; a scan of points near the stored ones, points in the 26 neighbours of the colliding voxels, and points in colliding
+    voxels absent from the map (a probe walks the whole chain, then stops at an empty slot)."""
+    keys = colliding_keys()
+    assert len(keys) >= n_map + n_absent
+    rng = np.random.default_rng(seed)
+    sel = keys[rng.permutation(len(keys))[:n_map + n_absent]]
+    present, absent = sel[:n_map], sel[n_map:]
+    corners = np.array([(0, 0, 0), (1, 0, 0), (0, 1, 0), (0, 0, 1), (1, 1, 1), (1, 1, 0), (0, 1, 1), (1, 0, 1)])[:cap] * 0.9 + 0.03
+    pts = np.concatenate([(k + _dyadic(corners + rng.uniform(0.0, 0.04, (cap, 3)), 2.0 ** -16)) * vs for k in present])
+    om = ko.OracleMap(vs, max_distance, cap)
+    om.add_points(pts)
+    assert om.num_points() == len(pts)
+    near = pts + _dyadic(0.03 * vs * rng.standard_normal(pts.shape), 2.0 ** -20)
+    shifts = np.array(SHIFTS[1:])
+    nbr = np.concatenate([(k + shifts[rng.permutation(26)[:8]] + rng.uniform(0.0, 1.0, (8, 3))) * vs for k in present])
+    miss = np.concatenate([(k + rng.uniform(0.0, 1.0, (4, 3))) * vs for k in absent])
+    scan = np.concatenate([near, nbr, miss])
+    sc = Scene("collide-%d-vs%g" % (n_map, vs), om, scan, IDENTITY.copy(), IDENTITY.copy(), 1.5 * vs, max_iter=3)
+    sc.present, sc.absent = present, absent
+    return sc
+
+
+def collision_scenes(ko):
+    return [collision_scene(ko, n, vs=vs, seed=13 + n) for n, vs in ((3, 1.0), (9, 0.5), (17, 0.3), (40, 1.0))]
+
+
+def nonfinite_rows(vs):
+    """Rows with NaN, +-Inf and +-3e9 vs in one or all coordinates (the reference's key of such a coordinate is INT_MIN), the
+    others inside voxel 0 so that a conversion that gave 0 for NaN would put the point into voxel (0, 0, 0)."""
+    bad = [NAN, INF, -INF, 3e9 * vs, -3e9 * vs]
+    rows = []
+    for b in bad:
+        for ax in range(3):
+            p = np.full(3, 0.25 * vs)
+            p[ax] = b
+            rows.append(p)
+        rows.append(np.full(3, b))
+    return np.array(rows)
+
+
+def with_nonfinite(pts, vs, seed=17):
+    """`pts` with the rows of nonfinite_rows() spread through it, NaN rows first (so that a NaN point comes first in voxel
+    (0, 0, 0) under a conversion that gives 0 for NaN), and a real point of voxel (0, 0, 0) after them."""
+    rng = np.random.default_rng(seed)
+    bad = nonfinite_rows(vs)
+    nan_first = np.array([[NAN, 0.25 * vs, 0.25 * vs], [NAN, NAN, NAN], [0.3 * vs, 0.3 * vs, 0.3 * vs]])
+    out = np.array(pts, dtype=np.float64, copy=True)
+    for row in bad:
+        i = int(rng.integers(0, len(out) + 1))
+        out = np.insert(out, i, row, axis=0)
+    return np.concatenate([nan_first, out])

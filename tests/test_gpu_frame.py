@@ -3,6 +3,7 @@ against the CPU oracle stage by stage: Preprocess + base transform, both VoxelDo
 import numpy as np
 import pytest
 
+import scenes as S
 from test_gpu_parity import TOL_R, TOL_T, gpu_map_from_oracle, sorted_voxels
 
 pytestmark = pytest.mark.gpu
@@ -128,3 +129,137 @@ def test_register_frame_edge_cases(oracle, gpu_ctx, workload):
     a = kb.RegisterFrame(gm2, w.scan, np.zeros(0), ident, ident, w.last_pose, w.rel_odom, w.tau, voxel_size=w.voxel_size)
     b = kb.RegisterFrame(gm3, w.scan, np.zeros(0), ident, ident, w.last_pose, w.rel_odom, w.tau, voxel_size=w.voxel_size, want_clouds=False)
     assert np.array_equal(a[0], b[0]) and b[1] == len(a[1]) and b[2] == len(a[2])
+
+
+def _frame_capi(kb, gm, frame, cap_frame, cap_source, voxel_size):
+    """kicp_register_frame with caller buffers of the given capacities (the Python wrapper always passes enough)."""
+    import ctypes as C
+    from kinematic_icp_b200 import _capi
+    from kinematic_icp_b200._capi import FrameInput, FrameParams, RegResult, dp
+    inp = FrameInput()
+    inp.data, inp.n, inp.dtype, inp.point_step = frame.ctypes.data, len(frame), _capi.KICP_DTYPE_F64, 0
+    fp = FrameParams()
+    fp.max_range, fp.min_range, fp.deskew, fp.voxel_size = 100.0, 0.5, 0, voxel_size
+    fp.reg.max_num_iterations, fp.reg.use_adaptive_odometry_regularization, fp.reg.convergence_criterion = 10, 1, 1e-3
+    ident = np.array([0, 0, 0, 1.0, 0, 0, 0])
+    out_pose, out_f, out_s = np.empty(7), np.empty((max(cap_frame, 1), 3)), np.empty((max(cap_source, 1), 3))
+    nf, ns, res = C.c_int64(), C.c_int64(), RegResult()
+    st = _capi.lib().kicp_register_frame(gm.h, C.byref(inp), dp(ident), dp(ident), dp(ident), dp(ident), 1.0, C.byref(fp), dp(out_pose),
+                                         dp(out_f), cap_frame, C.byref(nf), dp(out_s), cap_source, C.byref(ns), C.byref(res))
+    return st, nf.value, ns.value
+
+
+def test_register_frame_drive(oracle, monkeypatch):
+    """Twelve frames through kicp_register_frame on a context of their own and a map that starts at its smallest slab, each checked
+    against the oracle stage by stage: the preprocessed frame and the source bit for bit (1e-12 with de-skew), the pose to
+    1e-6 m / 1e-7 rad, the map bit for bit after the device's pose is replayed on the oracle's.  The drive holds a tiny frame followed
+    by one whose source exceeds max(2 x previous, 32 768) (the rest-of-source fetch, and a registration planned from a far smaller
+    frame), an empty frame and one with every point outside the range gate (NaN pose, flagged, map untouched), a frame that grows the
+    front end's scratch, growth of the map's slab inside the asynchronous update, de-skew, float32 and PointCloud2 layouts, and
+    frame_sync 0 and 1.  Then a caller buffer too small for the survivors: KICP_ERR_CAPACITY, the map unchanged, and
+    kicp_frame_clouds still holding the last frame's clouds."""
+    import ctypes as C
+
+    import kinematic_icp_b200 as kb
+    from kinematic_icp_b200 import _capi
+    ko = oracle
+    monkeypatch.setenv("KICP_MAP_VOXELS", "16384")
+    vs, md, cap, tau = 1.0, 40.0, 20, 1.0
+    rng = np.random.default_rng(2026)
+    world = np.c_[rng.uniform(-45.0, 85.0, 420_000), rng.uniform(-50.0, 50.0, 420_000), rng.uniform(-3.0, 12.0, 420_000)]
+    world = np.round(world * 4096.0) / 4096.0
+    ctx = kb.Context(0)
+    gm = kb.VoxelHashMap(ctx, vs, md, cap)
+    om = ko.OracleMap(vs, md, cap)
+    l2b = ko.se3_exp([0.1, 0.0, 0.2, 0.0, 0.0, 0.02])
+    step = ko.se3_exp([2.5, 0.1, 0.0, 0.0, 0.0, 0.01])
+    true_pose = ko.IDENTITY.copy()
+    last = ko.IDENTITY.copy()
+    # (kind, frame_sync): how each frame is built and handed over
+    plan = [("tiny", 0), ("big", 0), ("empty", 0), ("gated", 0), ("sub", 1), ("deskew", 0), ("f32", 0), ("pc2", 0), ("huge", 0), ("sub", 0),
+            ("deskew", 1), ("sub", 0)]
+    prev_source, last_clouds = 0, None
+    try:
+        for k, (kind, sync) in enumerate(plan):
+            odom = step if k else ko.IDENTITY.copy()
+            true_pose = ko.se3_compose(true_pose, odom)
+            lidar = ko.se3_transform(ko.se3_inverse(ko.se3_compose(true_pose, l2b)), world)  # the world in this frame's lidar frame
+            r = np.sqrt((lidar * lidar).sum(1))
+            lidar = lidar[(r < 100.0)]
+            stamps = np.zeros(0)
+            deskew_motion = ko.IDENTITY
+            if kind == "tiny":
+                frame = lidar[:150]
+            elif kind == "big":
+                frame = lidar
+            elif kind == "empty":
+                frame = np.zeros((0, 3))
+            elif kind == "gated":
+                frame = lidar[:3000] * 1e-4
+            elif kind == "huge":  # more points than any frame before: the scratch grows
+                frame = np.concatenate([lidar, lidar[::2] + 0.01])
+            else:
+                frame = lidar[k % 3::3]
+            if kind in ("f32", "pc2"):
+                frame = frame.astype(np.float32)
+            wide = frame.astype(np.float64)
+            if kind == "deskew":
+                stamps = np.linspace(7.0, 7.1, len(frame))
+                deskew_motion = ko.se3_compose(ko.se3_compose(ko.se3_inverse(l2b), odom), l2b)
+            ctx.set_option("frame_sync", sync)
+            if kind == "pc2":
+                rec = np.zeros(len(frame), dtype=[("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("i", "<f4")])
+                rec["x"], rec["y"], rec["z"], rec["i"] = frame[:, 0], frame[:, 1], frame[:, 2], 3.0
+                arg, extra = rec, dict(point_step=16, offsets=(0, 4, 8))
+            else:
+                arg, extra = frame, {}
+            before = sorted_voxels(*gm.export_voxels())
+            pose, g_frame, g_src, res = kb.RegisterFrame(gm, arg, stamps, deskew_motion, l2b, last, odom, tau, max_range=100.0, min_range=0.5,
+                                                         deskew=kind == "deskew", voxel_size=vs, **extra)
+            # the oracle, stage by stage
+            pre = ko.preprocess(wide, stamps, deskew_motion, 100.0, 0.5, kind == "deskew")
+            in_base = ko.se3_transform(l2b, pre) if len(pre) else np.zeros((0, 3))
+            fd = ko.voxel_downsample(in_base, 0.5 * vs) if len(in_base) else np.zeros((0, 3))
+            src = ko.voxel_downsample(fd, 1.5 * vs) if len(fd) else np.zeros((0, 3))
+            assert g_frame.shape == in_base.shape and g_src.shape == src.shape, kind
+            if kind == "deskew":
+                assert np.abs(g_frame - in_base).max() < 1e-12 and np.abs(g_src - src).max() < 1e-12
+            else:
+                assert S.same_bits(g_frame, in_base) and S.same_bits(g_src, src), kind
+            if kind == "big":
+                assert len(src) > max(2 * prev_source, 32768), (len(src), prev_source)
+            prev_source = len(src)
+            if len(src) == 0:  # nothing to register: the reference's NaN pose, flagged, the map untouched
+                assert np.isnan(pose).any() and res.status == kb.KICP_WARN_NO_CORRESPONDENCES, kind
+                after = sorted_voxels(*gm.export_voxels())
+                assert all(np.array_equal(a, b) for a, b in zip(before, after))
+                continue
+            # the oracle registers the device's source (bit-identical, or within 1e-12 under de-skew)
+            opose, ost = om.register(g_src, last, odom, tau)
+            assert res.status == 0 and res.iterations == ost.iterations, kind
+            dt, dr = ko.pose_delta(pose, opose)
+            assert dt < TOL_T and dr < TOL_R, (kind, dt, dr)
+            # the map received the device's frame_downsample at the device's pose
+            om.update_pose(ko.voxel_downsample(g_frame, 0.5 * vs), pose)
+            k1, c1, p1 = sorted_voxels(*gm.export_voxels())
+            k0, c0, p0 = sorted_voxels(*om.export_voxels())
+            assert np.array_equal(k1, k0) and np.array_equal(c1, c0) and S.same_bits(p1, p0), kind
+            last, last_clouds = pose, (g_frame, g_src)
+        assert gm.num_voxels() > 16384  # the slab grew during the drive
+        # a caller buffer too small for the survivors: KICP_ERR_CAPACITY before the map changes
+        ctx.set_option("frame_sync", 0)
+        before = sorted_voxels(*gm.export_voxels())
+        frame = np.ascontiguousarray(ko.se3_transform(ko.se3_inverse(ko.se3_compose(true_pose, l2b)), world[::50]))
+        st, nf, ns = _frame_capi(kb, gm, frame, 10, len(frame), vs)
+        assert st == _capi.KICP_ERR_CAPACITY and nf > 10
+        after = sorted_voxels(*gm.export_voxels())
+        assert all(S.same_bits(a, b) if a.dtype == np.float64 else np.array_equal(a, b) for a, b in zip(before, after))
+        fp_, fs_ = C.POINTER(C.c_double)(), C.POINTER(C.c_double)()
+        n_f, n_s = C.c_int64(), C.c_int64()
+        assert _capi.lib().kicp_frame_clouds(ctx.h, C.byref(fp_), C.byref(n_f), C.byref(fs_), C.byref(n_s)) == 0
+        got_f = np.ctypeslib.as_array(fp_, shape=(n_f.value * 3,)).reshape(-1, 3).copy()
+        got_s = np.ctypeslib.as_array(fs_, shape=(n_s.value * 3,)).reshape(-1, 3).copy()
+        assert S.same_bits(got_f, last_clouds[0]) and S.same_bits(got_s, last_clouds[1])
+    finally:
+        gm.close()
+        ctx.close()
