@@ -32,7 +32,79 @@ struct LaserTable {
     double2 *d_cs = nullptr;
     int64_t d_cap = 0;
     bool uploaded = false;
+    // no exception may cross the C ABI: without host memory for the table it is left invalid (the next scan recomputes)
+    int refresh(const kicp_laser_scan *scan) {
+        if (valid && n == scan->n && angle_min == scan->angle_min && angle_max == scan->angle_max) return KICP_OK;
+        try {
+            cs.resize((size_t)scan->n);
+        } catch (const std::exception &) {
+            valid = false, cs.clear(), cs.shrink_to_fit();
+            kicp_set_error("kicp_frame_stage_laser_scan: no host memory for the cos / sin table");
+            return KICP_ERR_CAPACITY;
+        }
+        valid = true, n = scan->n, angle_min = scan->angle_min, angle_max = scan->angle_max;
+        for (int64_t i = 0; i < n; ++i) {
+            const double angle = (double)scan->angle_min + (double)i * (double)scan->angle_increment;
+            cs[(size_t)i] = make_double2(std::cos(angle), std::sin(angle));
+        }
+        uploaded = false;
+        return KICP_OK;
+    }
+    int upload(cudaStream_t stream) {
+        if (uploaded) return KICP_OK;
+        if (d_cap < n) {
+            KICP_CUDA(cudaStreamSynchronize(stream));
+            cudaFree(d_cs);
+            d_cs = nullptr, d_cap = 0;
+            KICP_CUDA(cudaMalloc(&d_cs, (size_t)n * sizeof(double2)));
+            d_cap = n;
+        }
+        KICP_CUDA(cudaMemcpyAsync(d_cs, cs.data(), (size_t)n * sizeof(double2), cudaMemcpyHostToDevice, stream));
+        uploaded = true;
+        return KICP_OK;
+    }
 };
+
+// The two clouds RegisterFrame returns (frame and source), staged in pinned host memory for cap points each: as doubles, and with
+// KICP_STAGE_F32 as float32 records encoded on the device into d_rec (frame at 0, source at 3 cap; allocated on first use).  The
+// counts are what kicp_frame_clouds / kicp_frame_clouds_f32 return.
+struct Staging {
+    P3 *frame = nullptr, *source = nullptr;
+    float *d_rec = nullptr, *frame32 = nullptr, *source32 = nullptr;
+    int64_t cap = 0;
+    int64_t n_frame = 0, n_source = 0, n_frame32 = 0, n_source32 = 0;
+    int reserve(int64_t points, bool records) {
+        cap = points;
+        if (!frame) KICP_CUDA(cudaMallocHost(&frame, cap * sizeof(P3)));
+        if (!source) KICP_CUDA(cudaMallocHost(&source, cap * sizeof(P3)));
+        if (!records) return KICP_OK;
+        if (!d_rec) KICP_CUDA(cudaMalloc(&d_rec, (size_t)cap * 6 * sizeof(float)));
+        if (!frame32) KICP_CUDA(cudaMallocHost(&frame32, (size_t)cap * 3 * sizeof(float)));
+        if (!source32) KICP_CUDA(cudaMallocHost(&source32, (size_t)cap * 3 * sizeof(float)));
+        return KICP_OK;
+    }
+    void release() { cudaFreeHost(frame), cudaFreeHost(source), cudaFree(d_rec), cudaFreeHost(frame32), cudaFreeHost(source32); }
+    float *d_source_rec() const { return d_rec + 3 * cap; }
+    // copies on `copy` of frame[0, frame_n) and source[src_lo, src_hi) from the device clouds, as doubles (f64) and records (f32)
+    int fetch(cudaStream_t copy, const P3 *d_frame, const P3 *d_source, bool f64, bool f32, int64_t frame_n, int64_t src_lo,
+              int64_t src_hi) {
+        const size_t nf = (size_t)frame_n, lo = (size_t)src_lo, ns = (size_t)(src_hi - src_lo);
+        if (f64 && nf) KICP_CUDA(cudaMemcpyAsync(frame, d_frame, nf * sizeof(P3), cudaMemcpyDeviceToHost, copy));
+        if (f64 && ns) KICP_CUDA(cudaMemcpyAsync(source + lo, d_source + lo, ns * sizeof(P3), cudaMemcpyDeviceToHost, copy));
+        if (f32 && nf) KICP_CUDA(cudaMemcpyAsync(frame32, d_rec, nf * 3 * sizeof(float), cudaMemcpyDeviceToHost, copy));
+        if (f32 && ns)
+            KICP_CUDA(cudaMemcpyAsync(source32 + 3 * lo, d_source_rec() + 3 * lo, ns * 3 * sizeof(float), cudaMemcpyDeviceToHost, copy));
+        return KICP_OK;
+    }
+    // after the copy stream has drained: the staged counts, and the doubles to the caller's buffers (either may be null)
+    void publish(bool f64, bool f32, int64_t nf, int64_t ns, double *out_frame, double *out_source) {
+        if (f64) n_frame = nf, n_source = ns;
+        if (f32) n_frame32 = nf, n_source32 = ns;
+        if (out_frame && nf) memcpy(out_frame, frame, (size_t)nf * sizeof(P3));
+        if (out_source && ns) memcpy(out_source, source, (size_t)ns * sizeof(P3));
+    }
+};
+
 struct Scratch {
     P3 *in = nullptr, *out = nullptr, *out2 = nullptr, *out3 = nullptr;
     double *stamps = nullptr, *d_mm = nullptr;  // d_mm: {min, max} of the stamps, then the per-CTA partials of their reduction
@@ -44,12 +116,7 @@ struct Scratch {
     uint32_t *h_mapctr = nullptr;  // pinned, 8 words: the map's counters after an asynchronous update
     cudaEvent_t ev_front = nullptr;  // front end finished (the copy stream waits for it before staging the clouds)
     int64_t last_source = 0;       // registration-source points of the previous frame (sizes this frame's grid and staging copy)
-    P3 *h_frame = nullptr, *h_source = nullptr;  // pinned staging of the two clouds RegisterFrame returns (cap points each)
-    int64_t staged_frame = 0, staged_source = 0;
-    // KICP_STAGE_F32: the two clouds as float32 records, encoded on the device into d_rec (frame at 0, source at 3 cap) and staged in
-    // h_frame32 / h_source32 (cap points each); allocated on first use
-    float *d_rec = nullptr, *h_frame32 = nullptr, *h_source32 = nullptr;
-    int64_t staged_frame32 = 0, staged_source32 = 0;
+    Staging staged;
     // the frame kicp_frame_stage left in s.in (points) and s.stamps / s.d_mm (stamps and their {min, max}) for
     // kicp_register_staged_frame: its point count, -1 when there is none (consumed, or discarded by another front-end call)
     int64_t held_n = -1, held_n_stamps = 0;
@@ -62,8 +129,8 @@ struct Scratch {
 void release(Scratch &s) {
     cudaFree(s.in), cudaFree(s.out), cudaFree(s.out2), cudaFree(s.out3), cudaFree(s.stamps), cudaFree(s.d_mm_ticket);
     cudaFree(s.first_idx), cudaFree(s.slot_of), cudaFree(s.slots), cudaFree(s.d_count), cudaFree(s.d_mm);
-    cudaFree(s.raw), cudaFreeHost(s.h_count), cudaFreeHost(s.h_frame), cudaFreeHost(s.h_source), cudaFreeHost(s.h_mapctr), cudaFreeHost(s.h_range);
-    cudaFree(s.d_rec), cudaFreeHost(s.h_frame32), cudaFreeHost(s.h_source32);
+    cudaFree(s.raw), cudaFreeHost(s.h_count), cudaFreeHost(s.h_mapctr), cudaFreeHost(s.h_range);
+    s.staged.release();
     if (s.ev_front) cudaEventDestroy(s.ev_front);
     s = Scratch();
 }
@@ -110,22 +177,13 @@ int reserve(kicp_ctx *c, Scratch &s, int64_t n) {
     KICP_CUDA(cudaMallocHost(&s.h_mapctr, 8 * sizeof(uint32_t)));
     KICP_CUDA(cudaMallocHost(&s.h_range, 2 * sizeof(double)));
     KICP_CUDA(cudaEventCreateWithFlags(&s.ev_front, cudaEventDisableTiming));
-    KICP_CUDA(cudaMallocHost(&s.h_frame, cap * sizeof(P3)));
-    KICP_CUDA(cudaMallocHost(&s.h_source, cap * sizeof(P3)));
+    KICP_TRY(s.staged.reserve(cap, false));
     KICP_CUDA(cudaMalloc(&s.stamps, cap * sizeof(double)));
     KICP_CUDA(cudaMalloc(&s.first_idx, (size_t)nslots * sizeof(int)));
     KICP_CUDA(cudaMalloc(&s.slot_of, cap * sizeof(int)));
     KICP_CUDA(cudaMalloc(&s.slots, (size_t)nslots * sizeof(int4)));
     KICP_CUDA(cudaMalloc(&s.d_count, 4 * sizeof(int)));
     s.cap = cap, s.nslots = nslots;
-    return KICP_OK;
-}
-
-// the float32 staging of KICP_STAGE_F32, sized for s.cap points (freed with the rest of the scratch when it grows)
-int reserve_records(Scratch &s) {
-    if (!s.d_rec) KICP_CUDA(cudaMalloc(&s.d_rec, (size_t)s.cap * 6 * sizeof(float)));
-    if (!s.h_frame32) KICP_CUDA(cudaMallocHost(&s.h_frame32, (size_t)s.cap * 3 * sizeof(float)));
-    if (!s.h_source32) KICP_CUDA(cudaMallocHost(&s.h_source32, (size_t)s.cap * 3 * sizeof(float)));
     return KICP_OK;
 }
 
@@ -210,19 +268,18 @@ int enqueue_preprocess(kicp_ctx *c, Scratch &s, int n, const double *stamps, int
     KICP_CHECK_LAUNCH(c);
     return KICP_OK;
 }
-}  // namespace
 
-extern "C" int kicp_voxel_downsample(kicp_ctx *c, const double *xyz, int64_t n, double voxel_size, double *out_xyz, int64_t cap,
-                                     int64_t *m) {
-    if (c) scratch(c).held_n = -1;  // a staged frame (kicp_frame_stage) is discarded by any other front-end call
-    if (!c || !m || n < 0 || (n > 0 && (!xyz || !out_xyz)) || !(voxel_size > 0.0) || n > 0x3FFFFFFF) return KICP_ERR_INVALID;
-    *m = 0;
-    if (n == 0) return KICP_OK;
+// The opening of every front-end entry point: a frame staged by kicp_frame_stage is discarded — by a call that fails its validation
+// (`status`) too — then the device is set and the scratch reserved for n points.
+int open_frontend(kicp_ctx *c, int status, int64_t n) {
+    if (c) scratch(c).held_n = -1;
+    if (status != KICP_OK) return status;
     KICP_CUDA(cudaSetDevice(c->device));
-    Scratch &s = scratch(c);
-    KICP_TRY(reserve(c, s, n));
-    KICP_CUDA(cudaMemcpyAsync(s.in, xyz, (size_t)n * sizeof(P3), cudaMemcpyHostToDevice, c->stream));
-    KICP_TRY(enqueue_downsample(c, s, s.in, (int)n, nullptr, voxel_size, s.out, s.d_count));
+    return reserve(c, scratch(c), n);
+}
+
+// the survivor count in s.d_count, then the survivors in s.out when out_xyz holds them (kicp_voxel_downsample, kicp_preprocess)
+int read_back(kicp_ctx *c, Scratch &s, double *out_xyz, int64_t cap, int64_t *m) {
     int count = 0;
     KICP_CUDA(cudaMemcpyAsync(&count, s.d_count, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     KICP_CUDA(cudaStreamSynchronize(c->stream));
@@ -231,29 +288,33 @@ extern "C" int kicp_voxel_downsample(kicp_ctx *c, const double *xyz, int64_t n, 
     KICP_CUDA(cudaMemcpy(out_xyz, s.out, (size_t)count * sizeof(P3), cudaMemcpyDeviceToHost));
     return KICP_OK;
 }
+}  // namespace
+
+extern "C" int kicp_voxel_downsample(kicp_ctx *c, const double *xyz, int64_t n, double voxel_size, double *out_xyz, int64_t cap,
+                                     int64_t *m) {
+    const bool valid = c && m && n >= 0 && (n == 0 || (xyz && out_xyz)) && voxel_size > 0.0 && n <= 0x3FFFFFFF;
+    KICP_TRY(open_frontend(c, valid ? KICP_OK : KICP_ERR_INVALID, n));
+    *m = 0;
+    if (n == 0) return KICP_OK;
+    Scratch &s = scratch(c);
+    KICP_CUDA(cudaMemcpyAsync(s.in, xyz, (size_t)n * sizeof(P3), cudaMemcpyHostToDevice, c->stream));
+    KICP_TRY(enqueue_downsample(c, s, s.in, (int)n, nullptr, voxel_size, s.out, s.d_count));
+    return read_back(c, s, out_xyz, cap, m);
+}
 
 extern "C" int kicp_preprocess(kicp_ctx *c, const double *xyz, int64_t n, const double *stamps, int64_t n_stamps,
                                const double relative_motion[7], const double lidar_to_base[7], double max_range, double min_range,
                                int deskew, double *out_xyz, int64_t cap, int64_t *m) {
-    if (c) scratch(c).held_n = -1;
-    if (!c || !m || n < 0 || (n > 0 && (!xyz || !out_xyz)) || !relative_motion || !lidar_to_base || n > 0x3FFFFFFF)
-        return KICP_ERR_INVALID;
-    if (deskew && n_stamps > 0 && (n_stamps != n || !stamps)) return KICP_ERR_INVALID;
+    const bool valid = c && m && n >= 0 && (n == 0 || (xyz && out_xyz)) && relative_motion && lidar_to_base && n <= 0x3FFFFFFF &&
+                       !(deskew && n_stamps > 0 && (n_stamps != n || !stamps));
+    KICP_TRY(open_frontend(c, valid ? KICP_OK : KICP_ERR_INVALID, n));
     *m = 0;
     if (n == 0) return KICP_OK;
-    KICP_CUDA(cudaSetDevice(c->device));
     Scratch &s = scratch(c);
-    KICP_TRY(reserve(c, s, n));
     KICP_CUDA(cudaMemcpyAsync(s.in, xyz, (size_t)n * sizeof(P3), cudaMemcpyHostToDevice, c->stream));
     KICP_TRY(enqueue_preprocess(c, s, (int)n, stamps, n_stamps, false, relative_motion, lidar_to_base, max_range, min_range, deskew, s.out,
                                 s.d_count));
-    int count = 0;
-    KICP_CUDA(cudaMemcpyAsync(&count, s.d_count, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    KICP_CUDA(cudaStreamSynchronize(c->stream));
-    *m = count;
-    if (count > cap) return KICP_ERR_CAPACITY;
-    KICP_CUDA(cudaMemcpy(out_xyz, s.out, (size_t)count * sizeof(P3), cudaMemcpyDeviceToHost));
-    return KICP_OK;
+    return read_back(c, s, out_xyz, cap, m);
 }
 
 // ------------------------------------------------------------------------------------------- fused RegisterFrame
@@ -308,134 +369,109 @@ int enqueue_ingest(kicp_ctx *c, Scratch &s, const kicp_frame_input *in, const La
     return KICP_OK;
 }
 
+// The arguments of kicp_register_frame / kicp_register_staged_frame, for the frame they leave in s.in[0, n) with its stamps as
+// enqueue_preprocess takes them
+struct FrameArgs {
+    int64_t n;
+    const double *stamps;
+    int64_t n_stamps;
+    bool stamps_held;
+    const double *deskew_motion, *lidar_to_base, *last_pose, *relative_odometry;
+    double tau;
+    const kicp_frame_params *fp;
+    double *out_pose, *out_frame;
+    int64_t cap_frame, *n_frame;
+    double *out_source;
+    int64_t cap_source, *n_source;
+    kicp_reg_result *result;
+    std::chrono::steady_clock::time_point t0;  // the call's start (timing[] is measured from it)
+    bool valid() const {
+        return deskew_motion && lidar_to_base && last_pose && relative_odometry && fp && out_pose && fp->voxel_size > 0.0;
+    }
+};
+
 // KinematicICP::RegisterFrame from the frame in s.in[0, n) on: Preprocess, both down-samples, registration, map update, the two
-// clouds.  Stamps as enqueue_preprocess takes them.  Shared by kicp_register_frame and kicp_register_staged_frame.
-int register_ingested(kicp_map *map, Scratch &s, int64_t n, const double *stamps, int64_t n_stamps, bool stamps_held,
-                      const double deskew_motion[7], const double lidar_to_base[7], const double last_pose[7],
-                      const double relative_odometry[7], double tau, const kicp_frame_params *fp, double out_pose[7], double *out_frame,
-                      int64_t cap_frame, int64_t *n_frame, double *out_source, int64_t cap_source, int64_t *n_source,
-                      kicp_reg_result *result, std::chrono::steady_clock::time_point t0) {
-    auto ms_since = [&t0]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); };
+// clouds.  A frame is ONE host synchronisation (at its end): every later stage reads the survivor counts and the pose from device
+// memory, and the registration and the staging copies are sized by upper bounds.  The read-back order (read the counts back, size
+// everything exactly) remains for callers whose output buffers might be too small for the worst case — they are owed
+// KICP_ERR_CAPACITY before the map changes — and as option "frame_sync" for A/B measurements.
+int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
+    auto ms_since = [&a]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a.t0).count(); };
     kicp_ctx *c = map->ctx;
-    int counts[3] = {0, 0, 0};
+    const kicp_frame_params *fp = a.fp;
+    const int64_t n = a.n;
     // KICP_STAGE_F64 (and any other nonzero value but KICP_STAGE_F32 alone, as before the flag had two bits): the clouds as doubles
-    const bool stage = (fp->stage_clouds & ~KICP_STAGE_F32) != 0 || out_frame || out_source;
+    const bool stage = (fp->stage_clouds & ~KICP_STAGE_F32) != 0 || a.out_frame || a.out_source;
     const bool stage32 = (fp->stage_clouds & KICP_STAGE_F32) != 0;
+    const bool one_sync = n > 0 && !c->frame_sync && (!a.out_frame || a.cap_frame >= n) && (!a.out_source || a.cap_source >= n);
+    // the survivor counts of the three stages (12 bytes back, one synchronisation of the stream)
+    int counts[3] = {0, 0, 0};
+    auto read_counts = [&]() -> int {
+        KICP_CUDA(cudaMemcpyAsync(s.h_count, s.d_count, 3 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        KICP_CUDA(cudaStreamSynchronize(c->stream));
+        for (int k = 0; k < 3; ++k) counts[k] = s.h_count[k];
+        s.last_source = counts[2];
+        if (a.n_frame) *a.n_frame = counts[0];
+        if (a.n_source) *a.n_source = counts[2];
+        return KICP_OK;
+    };
     if (n > 0) {
         // s.out = preprocessed frame in base, s.out2 = frame_downsample (0.5 vs), s.out3 = source (1.5 vs); each stage reads
         // the previous stage's survivor count from device memory (KinematicICP.cpp:38-44, 54-62)
-        KICP_TRY(enqueue_preprocess(c, s, (int)n, stamps, n_stamps, stamps_held, deskew_motion, lidar_to_base, fp->max_range, fp->min_range,
-                                    fp->deskew, s.out, s.d_count));
+        KICP_TRY(enqueue_preprocess(c, s, (int)n, a.stamps, a.n_stamps, a.stamps_held, a.deskew_motion, a.lidar_to_base, fp->max_range,
+                                    fp->min_range, fp->deskew, s.out, s.d_count));
         KICP_TRY(enqueue_downsample(c, s, s.out, (int)n, s.d_count, fp->voxel_size * 0.5, s.out2, s.d_count + 1));
         KICP_TRY(enqueue_downsample(c, s, s.out2, (int)n, s.d_count + 1, fp->voxel_size * 1.5, s.out3, s.d_count + 2));
         if (stage32) {  // the published records, encoded before the registration so that they never share the SMs with its grid
-            KICP_TRY(reserve_records(s));
-            k_encode_clouds<<<(unsigned)((3 * n + 255) / 256), 256, 0, c->stream>>>(s.out, s.out3, (int)n, s.d_count, s.d_rec,
-                                                                                  s.d_rec + 3 * s.cap);
+            KICP_TRY(s.staged.reserve(s.cap, true));
+            k_encode_clouds<<<(unsigned)((3 * n + 255) / 256), 256, 0, c->stream>>>(s.out, s.out3, (int)n, s.d_count, s.staged.d_rec,
+                                                                                  s.staged.d_source_rec());
             KICP_CHECK_LAUNCH(c);
         }
-        // A frame is ONE host synchronisation (at its end): every later stage reads the survivor counts and the pose from device
-        // memory.  The legacy order (read the counts back, size everything exactly) remains for callers whose output buffers
-        // might be too small for the worst case — they are owed KICP_ERR_CAPACITY before the map changes — and as option
-        // "frame_sync" for A/B measurements.
-        const bool async_frame = !c->frame_sync && (!out_frame || cap_frame >= n) && (!out_source || cap_source >= n);
-        if (async_frame) {
-            s.timing[0] = ms_since();  // upload + front end enqueued
-            if (stage || stage32) KICP_CUDA(cudaEventRecord(s.ev_front, c->stream));
-            // registration of the source against the local map; the grid is sized from the previous frame's source
-            c->reg_n_hint = s.last_source > 0 ? s.last_source + s.last_source / 4 + 256 : 0;
-            KICP_TRY(kicp_enqueue_registration_device(map, reinterpret_cast<const double *>(s.out3), n, s.d_count + 2, last_pose,
-                                                      relative_odometry, tau, &fp->reg));
-            s.timing[1] = ms_since();  // + registration enqueued
-            // the two clouds go to pinned staging on the copy stream while the registration runs (sizes: upper bounds)
-            s.staged_frame = s.staged_source = 0;
-            s.staged_frame32 = s.staged_source32 = 0;
-            const int64_t src_copy = std::min<int64_t>(n, std::max<int64_t>(2 * s.last_source, 32768));
-            if (stage || stage32) KICP_CUDA(cudaStreamWaitEvent(c->copy_stream, s.ev_front, 0));
-            if (stage) {
-                KICP_CUDA(cudaMemcpyAsync(s.h_frame, s.out, (size_t)n * sizeof(P3), cudaMemcpyDeviceToHost, c->copy_stream));
-                KICP_CUDA(cudaMemcpyAsync(s.h_source, s.out3, (size_t)src_copy * sizeof(P3), cudaMemcpyDeviceToHost, c->copy_stream));
-            }
-            if (stage32) {
-                KICP_CUDA(cudaMemcpyAsync(s.h_frame32, s.d_rec, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost, c->copy_stream));
-                KICP_CUDA(cudaMemcpyAsync(s.h_source32, s.d_rec + 3 * s.cap, (size_t)src_copy * 3 * sizeof(float), cudaMemcpyDeviceToHost,
-                                          c->copy_stream));
-            }
-            // local_map_.Update(frame_downsample, new_pose) (KinematicICP.cpp:79), pose and count still on the device; a NaN pose
-            // (zero correspondences, which the reference does not defend against) leaves the map untouched
-            KICP_TRY(kicp_map_update_pose_async(map, reinterpret_cast<const double *>(s.out2), n, s.d_count + 1, kicp_device_result(c),
-                                                s.h_mapctr));
-            KICP_CUDA(cudaMemcpyAsync(s.h_count, s.d_count, 3 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-            KICP_CUDA(cudaStreamSynchronize(c->stream));  // THE synchronisation of the frame
-            s.timing[2] = s.timing[3] = ms_since();      // + registration and map update finished
-            for (int k = 0; k < 3; ++k) counts[k] = s.h_count[k];
-            s.last_source = counts[2];
-            const kicp_reg_result &r = *c->h_result;
-            for (int k = 0; k < 7; ++k) out_pose[k] = r.pose[k];
-            if (result) *result = r;
-            int status = r.status;
-            const int mst = kicp_map_finish_update(map, s.h_mapctr);
-            if (mst != KICP_OK) status = mst;
-            if (n_frame) *n_frame = counts[0];
-            if (n_source) *n_source = counts[2];
-            // the source outgrew the previous frame's twofold: fetch the rest
-            if (stage && counts[2] > src_copy)
-                KICP_CUDA(cudaMemcpyAsync(s.h_source + src_copy, s.out3 + src_copy, (size_t)(counts[2] - src_copy) * sizeof(P3),
-                                          cudaMemcpyDeviceToHost, c->copy_stream));
-            if (stage32 && counts[2] > src_copy)
-                KICP_CUDA(cudaMemcpyAsync(s.h_source32 + 3 * src_copy, s.d_rec + 3 * s.cap + 3 * src_copy,
-                                          (size_t)(counts[2] - src_copy) * 3 * sizeof(float), cudaMemcpyDeviceToHost, c->copy_stream));
-            if (stage || stage32) KICP_CUDA(cudaStreamSynchronize(c->copy_stream));
-            if (stage) {
-                s.staged_frame = counts[0], s.staged_source = counts[2];
-                if (out_frame && counts[0]) memcpy(out_frame, s.h_frame, (size_t)counts[0] * sizeof(P3));
-                if (out_source && counts[2]) memcpy(out_source, s.h_source, (size_t)counts[2] * sizeof(P3));
-            }
-            if (stage32) s.staged_frame32 = counts[0], s.staged_source32 = counts[2];
-            s.timing[4] = ms_since();  // + clouds delivered
-            return status;
-        }
-        KICP_CUDA(cudaMemcpyAsync(s.h_count, s.d_count, 3 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        KICP_CUDA(cudaStreamSynchronize(c->stream));  // legacy order: 12 bytes back, sizes the registration grid exactly
-        for (int k = 0; k < 3; ++k) counts[k] = s.h_count[k];
-        s.last_source = counts[2];
+        if (!one_sync) KICP_TRY(read_counts());
     }
     s.timing[0] = ms_since();  // upload + front end (ingest, de-skew, filter, transform, both down-samples)
-    if (n_frame) *n_frame = counts[0];
-    if (n_source) *n_source = counts[2];
-    if ((out_frame && counts[0] > cap_frame) || (out_source && counts[2] > cap_source)) return KICP_ERR_CAPACITY;
-    // registration of the source against the local map, enqueued first so that the downloads below overlap it
-    KICP_TRY(kicp_enqueue_registration_device(map, counts[2] ? reinterpret_cast<const double *>(s.out3) : nullptr, counts[2], nullptr,
-                                              last_pose, relative_odometry, tau, &fp->reg));
+    // (in the single-synchronisation order the counts are still 0 and the caller's buffers hold n points)
+    if ((a.out_frame && counts[0] > a.cap_frame) || (a.out_source && counts[2] > a.cap_source)) return KICP_ERR_CAPACITY;
+    if (one_sync) {
+        if (stage || stage32) KICP_CUDA(cudaEventRecord(s.ev_front, c->stream));
+        c->reg_n_hint = s.last_source > 0 ? s.last_source + s.last_source / 4 + 256 : 0;  // the grid is planned from the previous source
+    }
+    // registration of the source against the local map, enqueued first so that the staging copies overlap it
+    const int64_t reg_n = one_sync ? n : counts[2];
+    KICP_TRY(kicp_enqueue_registration_device(map, reg_n ? reinterpret_cast<const double *>(s.out3) : nullptr, reg_n,
+                                              one_sync ? s.d_count + 2 : nullptr, a.last_pose, a.relative_odometry, a.tau, &fp->reg));
     s.timing[1] = ms_since();  // + registration enqueued
-    // the two clouds go to pinned staging on the copy stream while the registration runs (the records were encoded before the
-    // synchronisation above)
-    s.staged_frame = s.staged_source = 0;
-    s.staged_frame32 = s.staged_source32 = 0;
-    if (stage && counts[0]) KICP_CUDA(cudaMemcpyAsync(s.h_frame, s.out, (size_t)counts[0] * sizeof(P3), cudaMemcpyDeviceToHost, c->copy_stream));
-    if (stage && counts[2])
-        KICP_CUDA(cudaMemcpyAsync(s.h_source, s.out3, (size_t)counts[2] * sizeof(P3), cudaMemcpyDeviceToHost, c->copy_stream));
-    if (stage32 && counts[0])
-        KICP_CUDA(cudaMemcpyAsync(s.h_frame32, s.d_rec, (size_t)counts[0] * 3 * sizeof(float), cudaMemcpyDeviceToHost, c->copy_stream));
-    if (stage32 && counts[2])
-        KICP_CUDA(cudaMemcpyAsync(s.h_source32, s.d_rec + 3 * s.cap, (size_t)counts[2] * 3 * sizeof(float), cudaMemcpyDeviceToHost,
-                                  c->copy_stream));
-    KICP_CUDA(cudaStreamSynchronize(c->stream));
+    // the two clouds go to pinned staging on the copy stream while the registration runs; in the single-synchronisation order the
+    // frame is copied for n points and the source for the previous frame's twofold (the rest follows below)
+    s.staged.n_frame = s.staged.n_source = s.staged.n_frame32 = s.staged.n_source32 = 0;
+    const int64_t src_copy = one_sync ? std::min<int64_t>(n, std::max<int64_t>(2 * s.last_source, 32768)) : counts[2];
+    if (one_sync && (stage || stage32)) KICP_CUDA(cudaStreamWaitEvent(c->copy_stream, s.ev_front, 0));
+    KICP_TRY(s.staged.fetch(c->copy_stream, s.out, s.out3, stage, stage32, one_sync ? n : counts[0], 0, src_copy));
+    if (one_sync) {
+        // local_map_.Update(frame_downsample, new_pose) (KinematicICP.cpp:79), pose and count still on the device
+        KICP_TRY(kicp_map_update_pose_async(map, reinterpret_cast<const double *>(s.out2), n, s.d_count + 1, kicp_device_result(c),
+                                            s.h_mapctr));
+        KICP_TRY(read_counts());  // THE synchronisation of the frame
+    } else {
+        KICP_CUDA(cudaStreamSynchronize(c->stream));
+    }
     s.timing[2] = ms_since();  // + registration finished
     const kicp_reg_result &r = *c->h_result;
-    for (int k = 0; k < 7; ++k) out_pose[k] = r.pose[k];
-    if (result) *result = r;
+    for (int k = 0; k < 7; ++k) a.out_pose[k] = r.pose[k];
+    if (a.result) *a.result = r;
     int status = r.status;
-    // local_map_.Update(frame_downsample, new_pose) (KinematicICP.cpp:79); a NaN pose (zero correspondences, which the
-    // reference does not defend against) is reported and leaves the map untouched
-    if (status == KICP_OK && counts[1] > 0)
+    // a NaN pose (zero correspondences, which the reference does not defend against) is reported and leaves the map untouched
+    if (one_sync) {
+        const int mst = kicp_map_finish_update(map, s.h_mapctr);
+        if (mst != KICP_OK) status = mst;
+    } else if (status == KICP_OK && counts[1] > 0) {
         status = kicp_map_update_pose_device(map, reinterpret_cast<const double *>(s.out2), counts[1], r.pose);
+    }
     s.timing[3] = ms_since();  // + map update
-    KICP_CUDA(cudaStreamSynchronize(c->copy_stream));
-    if (stage) s.staged_frame = counts[0], s.staged_source = counts[2];
-    if (stage32) s.staged_frame32 = counts[0], s.staged_source32 = counts[2];
-    if (out_frame && counts[0]) memcpy(out_frame, s.h_frame, (size_t)counts[0] * sizeof(P3));
-    if (out_source && counts[2]) memcpy(out_source, s.h_source, (size_t)counts[2] * sizeof(P3));
+    if (counts[2] > src_copy) KICP_TRY(s.staged.fetch(c->copy_stream, s.out, s.out3, stage, stage32, 0, src_copy, counts[2]));
+    if (stage || stage32 || !one_sync) KICP_CUDA(cudaStreamSynchronize(c->copy_stream));
+    s.staged.publish(stage, stage32, counts[0], counts[2], a.out_frame, a.out_source);
     s.timing[4] = ms_since();  // + clouds delivered
     return status;
 }
@@ -449,25 +485,18 @@ extern "C" int kicp_register_frame(kicp_map *map, const kicp_frame_input *in, co
                                    const double last_pose[7], const double relative_odometry[7], double tau, const kicp_frame_params *fp,
                                    double out_pose[7], double *out_frame, int64_t cap_frame, int64_t *n_frame, double *out_source,
                                    int64_t cap_source, int64_t *n_source, kicp_reg_result *result) {
-    if (map) scratch(map->ctx).held_n = -1;
-    if (!map || !in || !deskew_motion || !lidar_to_base || !last_pose || !relative_odometry || !fp || !out_pose) return KICP_ERR_INVALID;
+    const FrameArgs a{in ? in->n : 0, in ? in->stamps : nullptr, in ? in->n_stamps : 0, false, deskew_motion, lidar_to_base, last_pose,
+                      relative_odometry, tau, fp, out_pose, out_frame, cap_frame, n_frame, out_source, cap_source, n_source, result,
+                      std::chrono::steady_clock::now()};
     Layout l;
-    if (frame_layout(in, l) != KICP_OK || !(fp->voxel_size > 0.0)) return KICP_ERR_INVALID;
-    const int64_t n = in->n;
-    const int deskew = fp->deskew && in->n_stamps > 0;
-    if (deskew && (in->n_stamps != n || !in->stamps)) return KICP_ERR_INVALID;
+    const bool valid = map && in && a.valid() && frame_layout(in, l) == KICP_OK &&
+                       !(fp->deskew && a.n_stamps > 0 && (a.n_stamps != a.n || !a.stamps));
+    KICP_TRY(open_frontend(map ? map->ctx : nullptr, valid ? KICP_OK : KICP_ERR_INVALID, a.n));
     if (n_frame) *n_frame = 0;
     if (n_source) *n_source = 0;
-    const auto t0 = std::chrono::steady_clock::now();
-    kicp_ctx *c = map->ctx;
-    KICP_CUDA(cudaSetDevice(c->device));
-    Scratch &s = scratch(c);
-    if (n > 0) {
-        KICP_TRY(reserve(c, s, n));
-        KICP_TRY(enqueue_ingest(c, s, in, l, nullptr));
-    }
-    return register_ingested(map, s, n, in->stamps, in->n_stamps, false, deskew_motion, lidar_to_base, last_pose, relative_odometry, tau, fp,
-                             out_pose, out_frame, cap_frame, n_frame, out_source, cap_source, n_source, result, t0);
+    Scratch &s = scratch(map->ctx);
+    if (a.n > 0) KICP_TRY(enqueue_ingest(map->ctx, s, in, l, nullptr));
+    return register_ingested(map, s, a);
 }
 
 // The first half of an online node's frame (LidarOdometryServer.cpp:186-210 needs the sweep's stamps before it can look up the
@@ -475,26 +504,23 @@ extern "C" int kicp_register_frame(kicp_map *map, const kicp_frame_input *in, co
 // 16 bytes come back.  The frame stays in HBM for kicp_register_staged_frame.
 extern "C" int kicp_frame_stage(kicp_ctx *c, const kicp_frame_input *in, int32_t stamp_datatype, int32_t stamp_offset,
                                 double stamp_range[2], int64_t *n_stamps) {
-    if (c) scratch(c).held_n = -1;
-    if (!c || !in || !stamp_range || !n_stamps) return KICP_ERR_INVALID;
     Layout l;
-    if (frame_layout(in, l) != KICP_OK) return KICP_ERR_INVALID;
-    const int64_t n = in->n;
-    StampArgs t{stamp_datatype, stamp_offset};
-    if (stamp_datatype != 0) {
+    auto validate = [&]() -> int {
+        if (!c || !in || !stamp_range || !n_stamps || frame_layout(in, l) != KICP_OK) return KICP_ERR_INVALID;
+        if (stamp_datatype == 0) return in->n_stamps > 0 && (in->n_stamps != in->n || !in->stamps) ? KICP_ERR_INVALID : KICP_OK;
         if (stamp_datatype != 6 && stamp_datatype != 7 && stamp_datatype != 8) return KICP_ERR_UNSUPPORTED;
         const int width = stamp_datatype == 8 ? 8 : 4;
         if (in->point_step <= 0 || stamp_offset < 0 || stamp_offset + width > in->point_step || in->n_stamps > 0) return KICP_ERR_INVALID;
-    } else if (in->n_stamps > 0 && (in->n_stamps != n || !in->stamps)) {
-        return KICP_ERR_INVALID;
-    }
-    KICP_CUDA(cudaSetDevice(c->device));
+        return KICP_OK;
+    };
+    KICP_TRY(open_frontend(c, validate(), in ? in->n : 0));
+    const int64_t n = in->n;
+    const StampArgs t{stamp_datatype, stamp_offset};
     Scratch &s = scratch(c);
     stamp_range[0] = stamp_range[1] = 0.0;
     *n_stamps = 0;
     const int64_t stamps = n > 0 && (stamp_datatype != 0 || in->n_stamps > 0) ? n : 0;
     if (n > 0) {
-        KICP_TRY(reserve(c, s, n));
         KICP_TRY(enqueue_ingest(c, s, in, l, stamp_datatype != 0 ? &t : nullptr));
         if (stamps) {
             if (stamp_datatype == 0)
@@ -514,44 +540,17 @@ extern "C" int kicp_frame_stage(kicp_ctx *c, const kicp_frame_input *in, int32_t
 // compacts them into the staged frame (s.in, s.stamps), k_stamp_minmax reduces the beam-indexed stamps it leaves in s.out; the range
 // and the kept count come back with one host synchronisation.
 extern "C" int kicp_frame_stage_laser_scan(kicp_ctx *c, const kicp_laser_scan *scan, double stamp_range[2], int64_t *n_points) {
-    if (c) scratch(c).held_n = -1;
-    if (!c || !scan || !stamp_range || !n_points) return KICP_ERR_INVALID;
+    const bool valid = c && scan && stamp_range && n_points && scan->n >= 0 && scan->n <= 0x3FFFFFFF && (scan->n == 0 || scan->ranges);
+    KICP_TRY(open_frontend(c, valid ? KICP_OK : KICP_ERR_INVALID, valid ? scan->n : 0));
     const int64_t n = scan->n;
-    if (n < 0 || n > 0x3FFFFFFF || (n > 0 && !scan->ranges)) return KICP_ERR_INVALID;
-    KICP_CUDA(cudaSetDevice(c->device));
     Scratch &s = scratch(c);
     stamp_range[0] = stamp_range[1] = 0.0;
     *n_points = 0;
     LaserTable &lt = frontend(c).laser;
-    if (!lt.valid || lt.n != n || lt.angle_min != scan->angle_min || lt.angle_max != scan->angle_max) {
-        try {
-            lt.cs.resize((size_t)n);
-        } catch (const std::exception &) {  // no exception may cross the C ABI; the table is left invalid, so the next scan recomputes
-            lt.valid = false, lt.cs.clear(), lt.cs.shrink_to_fit();
-            kicp_set_error("kicp_frame_stage_laser_scan: no host memory for the cos / sin table");
-            return KICP_ERR_CAPACITY;
-        }
-        lt.valid = true, lt.n = n, lt.angle_min = scan->angle_min, lt.angle_max = scan->angle_max;
-        for (int64_t i = 0; i < n; ++i) {
-            const double angle = (double)scan->angle_min + (double)i * (double)scan->angle_increment;
-            lt.cs[(size_t)i] = make_double2(std::cos(angle), std::sin(angle));
-        }
-        lt.uploaded = false;
-    }
+    KICP_TRY(lt.refresh(scan));
     int64_t kept = 0;
     if (n > 0) {
-        KICP_TRY(reserve(c, s, n));
-        if (!lt.uploaded) {
-            if (lt.d_cap < n) {
-                KICP_CUDA(cudaStreamSynchronize(c->stream));
-                cudaFree(lt.d_cs);
-                lt.d_cs = nullptr, lt.d_cap = 0;
-                KICP_CUDA(cudaMalloc(&lt.d_cs, (size_t)n * sizeof(double2)));
-                lt.d_cap = n;
-            }
-            KICP_CUDA(cudaMemcpyAsync(lt.d_cs, lt.cs.data(), (size_t)n * sizeof(double2), cudaMemcpyHostToDevice, c->stream));
-            lt.uploaded = true;
-        }
+        KICP_TRY(lt.upload(c->stream));
         KICP_TRY(reserve_raw(c, s, (size_t)n * sizeof(float)));
         KICP_CUDA(cudaMemcpyAsync(s.raw, scan->ranges, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
         double *beam_stamps = reinterpret_cast<double *>(s.out);  // n doubles; s.out is free until the registration's Preprocess
@@ -579,36 +578,32 @@ extern "C" int kicp_register_staged_frame(kicp_map *map, const double deskew_mot
                                           double *out_frame, int64_t cap_frame, int64_t *n_frame, double *out_source, int64_t cap_source,
                                           int64_t *n_source, kicp_reg_result *result) {
     if (!map) return KICP_ERR_INVALID;
-    kicp_ctx *c = map->ctx;
-    Scratch &s = scratch(c);
-    const int64_t n = s.held_n;
-    s.held_n = -1;  // consumed, whatever the outcome
-    if (n < 0 || !deskew_motion || !lidar_to_base || !last_pose || !relative_odometry || !fp || !out_pose || !(fp->voxel_size > 0.0))
-        return KICP_ERR_INVALID;
+    Scratch &s = scratch(map->ctx);
+    const FrameArgs a{s.held_n, nullptr, s.held_n_stamps, true, deskew_motion, lidar_to_base, last_pose, relative_odometry, tau, fp,
+                      out_pose, out_frame, cap_frame, n_frame, out_source, cap_source, n_source, result, std::chrono::steady_clock::now()};
+    // the staged frame is consumed, whatever the outcome (its points are in the scratch already)
+    KICP_TRY(open_frontend(map->ctx, a.n >= 0 && a.valid() ? KICP_OK : KICP_ERR_INVALID, a.n));
     if (n_frame) *n_frame = 0;
     if (n_source) *n_source = 0;
-    const auto t0 = std::chrono::steady_clock::now();
-    KICP_CUDA(cudaSetDevice(c->device));
-    return register_ingested(map, s, n, nullptr, s.held_n_stamps, true, deskew_motion, lidar_to_base, last_pose, relative_odometry, tau, fp,
-                             out_pose, out_frame, cap_frame, n_frame, out_source, cap_source, n_source, result, t0);
+    return register_ingested(map, s, a);
 }
 
 /* The clouds of the last kicp_register_frame on this context (fp->stage_clouds), in context-owned pinned host memory, valid
  * until the next kicp_register_frame / kicp_preprocess / kicp_voxel_downsample call on the same context. */
 extern "C" int kicp_frame_clouds(kicp_ctx *c, const double **frame, int64_t *n_frame, const double **source, int64_t *n_source) {
     if (!c || !frame || !n_frame || !source || !n_source) return KICP_ERR_INVALID;
-    Scratch &s = scratch(c);
-    *frame = reinterpret_cast<const double *>(s.h_frame), *n_frame = s.staged_frame;
-    *source = reinterpret_cast<const double *>(s.h_source), *n_source = s.staged_source;
+    const Staging &st = scratch(c).staged;
+    *frame = reinterpret_cast<const double *>(st.frame), *n_frame = st.n_frame;
+    *source = reinterpret_cast<const double *>(st.source), *n_source = st.n_source;
     return KICP_OK;
 }
 
 // The same clouds as float32 records (fp->stage_clouds & KICP_STAGE_F32), encoded on the device; same lifetime
 extern "C" int kicp_frame_clouds_f32(kicp_ctx *c, const float **frame, int64_t *n_frame, const float **source, int64_t *n_source) {
     if (!c || !frame || !n_frame || !source || !n_source) return KICP_ERR_INVALID;
-    Scratch &s = scratch(c);
-    *frame = s.h_frame32, *n_frame = s.staged_frame32;
-    *source = s.h_source32, *n_source = s.staged_source32;
+    const Staging &st = scratch(c).staged;
+    *frame = st.frame32, *n_frame = st.n_frame32;
+    *source = st.source32, *n_source = st.n_source32;
     return KICP_OK;
 }
 
