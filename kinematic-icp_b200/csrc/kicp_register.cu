@@ -309,11 +309,12 @@ __device__ __forceinline__ unsigned *class_entry(const KernelArgs &a, int n, int
     return base + ((c & 1) ? pos : (unsigned)n - 1u - pos);
 }
 
-// gate, residual, Jacobian and the seven sums of one correspondence (Registration.cpp:75, 86-93, 110-118)
+// gate, residual, Jacobian and the seven sums of one correspondence (Registration.cpp:75, 86-93, 110-118).  rr is the caller's
+// dist2 of the pair: the reference's own square, so the gate sqrt(rr) < tau is its (neighbor - query).norm() < tau bit for bit (a
+// square recomputed here would be contracted, and a point at tau could fall on the other side); Σ|r|^2 sums the same squares.
 __device__ __forceinline__ void accumulate(WarpSm &sm, int lane, const PoseState &ps, double nx, double ny, double nz, double qx, double qy,
-                                           double qz, double px, double py) {
+                                           double qz, double px, double py, double rr) {
     const double rx = qx - nx, ry = qy - ny, rz = qz - nz;  // r = T p - n
-    const double rr = rx * rx + ry * ry + rz * rz;
     if (sqrt(rr) < ps.tau) {  // distance < max_correspondance_distance   (Registration.cpp:75)
         // J = [R e_x | R (-p_y, p_x, 0)]      (Registration.cpp:89-91)
         const double c0x = ps.R[0], c0y = ps.R[3], c0z = ps.R[6];
@@ -430,8 +431,9 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                           ovz = voxel_of(oz, vs, inv_vs, a.pow2_voxel);
                 const double mx = qx - ox, my = qy - oy, mz = qz - oz;
                 const double delta = sqrt(mx * mx + my * my + mz * mz) * (1.0 + 1e-9) + 1e-12;
-                const double d1 = sqrt(dist2(c1.x, c1.y, c1.z, qx, qy, qz));
-                const double d2 = have2 ? sqrt(dist2(c2.x, c2.y, c2.z, qx, qy, qz)) : DBL_MAX;
+                const double s1 = dist2(c1.x, c1.y, c1.z, qx, qy, qz);
+                const double s2 = have2 ? dist2(c2.x, c2.y, c2.z, qx, qy, qz) : DBL_MAX;
+                const double d1 = sqrt(s1), d2 = have2 ? sqrt(s2) : DBL_MAX;
                 // the two remembered candidates may have swapped; a near-tie between them is left to the search (only it applies the
                 // reference's visiting-order rule)
                 const bool second_wins = d2 < d1;
@@ -461,7 +463,7 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                 if (cert) {
                     a.nn_l[i] = __double2float_rz(room * (1.0 - 1e-7));
                     if (second_wins) a.nn_g[i] = g2, a.nn_g2[i] = g1;
-                    if (haveg) accumulate(sm, lane, s_ps, c.x, c.y, c.z, qx, qy, qz, px, py);
+                    if (haveg) accumulate(sm, lane, s_ps, c.x, c.y, c.z, qx, qy, qz, px, py, second_wins ? s2 : s1);
                 }
                 // Everything else is searched again.  The old neighbour bounds that search if it is one of the new 27 voxels' points; with
                 // few neighbour voxels inside the bound the search is ONE merged stage, else it is staged.  The point goes to the list
@@ -688,6 +690,7 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                     const bool act = more && lane < tpb && base + lane < total;
                     const unsigned okpack = act ? (unsigned)sm.task[base + lane] : 0u;
                     uint32_t meta = KICP_SLOT_EMPTY;
+                    bool kmin = false;  // a key coordinate is INT_MIN
                     if (more) {
                         KR_PROF_COUNT(9)
                         const int o = (int)(okpack >> 5), k = (int)(okpack & 31u);
@@ -720,9 +723,17 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                                 }
                             }
                         }
+                        kmin = min(min(kx, ky), kz) == INT_MIN;
                     }
                     KR_PROF(2)
                     // -------------------------------------------------------- number the 128-byte lines of the batch
+                    // The voxel's min_element starts from its first point and replaces it only by a point at a smaller distance: a first
+                    // point with a NaN coordinate (NaN distance to every query) is never replaced, and the comparison across voxels never
+                    // takes it — the reference finds nothing in that voxel.  A NaN coordinate has the key INT_MIN: only such are looked at.
+                    if (kmin && meta != KICP_SLOT_EMPTY) {
+                        const double *p0 = a.map.pts + (size_t)(meta >> 8) * (size_t)a.map.cap * KICP_PSTRIDE;
+                        if (isnan(__ldg(p0)) || isnan(__ldg(p0 + 1)) || isnan(__ldg(p0 + 2))) meta = KICP_SLOT_EMPTY;
+                    }
                     const int cnt = meta == KICP_SLOT_EMPTY ? 0 : (int)(meta & 0xFFu);
                     const int nl = (cnt + 3) >> 2;
                     int incl = nl;
@@ -839,15 +850,16 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                 double dj[4];
 #pragma unroll
                 for (int j = 0; j < 4; ++j) dj[j] = dist2(cc[j].x, cc[j].y, cc[j].z, q0.x, q0.y, q0z);
-                int jw = 0;
+                int jw = 0;  // (a NaN distance is the line's minimum never: a point before the minimum at NaN gives way to it)
 #pragma unroll
                 for (int j = 1; j < 4; ++j)
-                    if (j < (int)bvalid && closer(dj[j], dj[jw])) jw = j;
+                    if (j < (int)bvalid && (closer(dj[j], dj[jw]) || dj[jw] != dj[jw])) jw = j;
                 Point4 c = cc[0];
+                double dw = dj[0];
 #pragma unroll
                 for (int j = 1; j < 4; ++j)
-                    if (jw == j) c = cc[j];
-                if (have) accumulate(sm, lane, s_ps, c.x, c.y, c.z, q0.x, q0.y, q0z, sm.px[lane], sm.py[lane]);
+                    if (jw == j) c = cc[j], dw = dj[j];
+                if (have) accumulate(sm, lane, s_ps, c.x, c.y, c.z, q0.x, q0.y, q0z, sm.px[lane], sm.py[lane], dw);
                 if (cache && valid) {
                     // What the next pass may rely on: the neighbour g1, the runner-up g2 among the points of the two best lines, and
                     // l = how far every OTHER candidate is at least (third point of those lines, every other line, skipped cubes).
