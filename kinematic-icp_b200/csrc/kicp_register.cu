@@ -51,17 +51,17 @@
 using namespace kicp_dev;
 
 #ifndef KR_WARPS
-#define KR_WARPS 10                   // warps per CTA (2 x 10 warps per SM; 64 K registers and 228 KB of shared memory per SM)
+#define KR_WARPS 8                    // warps per CTA (3 x 8 warps per SM; 64 K registers and 228 KB of shared memory per SM)
 #endif
 #define KR_THREADS (KR_WARPS * 32)
 #ifndef KR_MINB
-#define KR_MINB 2                     // resident CTAs per SM the kernel is compiled for (a larger L1 rather than more warps)
+#define KR_MINB 3                     // resident CTAs per SM the kernel is compiled for (80 registers: 24 warps hide more latency)
 #endif
 #ifndef KR_LCAP
 #define KR_LCAP 192                   // lines the per-warp buffer holds (a batch of 32 tasks adds at most 160 at 20 points per voxel)
 #endif
 #ifndef KR_G
-#define KR_G 3                        // line-rounds (of 8 lines = 32 points) in flight together (96 registers at 2 x 320 threads)
+#define KR_G 3                        // line-rounds (of 8 lines = 32 points) in flight together
 #endif
 #ifndef KR_MERGE_MAX
 #define KR_MERGE_MAX 19               // neighbour voxels a seeded point may bring into its single merged stage (20 tasks x 32 owners = KR_TCAP)
@@ -248,17 +248,6 @@ __device__ __forceinline__ void load_scan_point(const ScanView &sv, int i, doubl
     }
 }
 
-// per-lane work counters (option "stats") -> warp sum -> one atomic per warp
-__device__ __forceinline__ void stats_flush(RegState *st, unsigned long long probes, unsigned long long cands, unsigned long long lines) {
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-        probes += __shfl_xor_sync(0xFFFFFFFFu, probes, d);
-        cands += __shfl_xor_sync(0xFFFFFFFFu, cands, d);
-        lines += __shfl_xor_sync(0xFFFFFFFFu, lines, d);
-    }
-    if ((threadIdx.x & 31) == 0) atomicAdd(&st->stats[0], probes), atomicAdd(&st->stats[1], cands), atomicAdd(&st->stats[2], lines);
-}
-
 // The shifts of one search stage that survive the exact bound (bit k <-> voxel_shifts[k]).  Stage 0: the own voxel;
 // stage 1: the 6 faces; stage 2: the 12 edges and 8 corners, pruned with the best the faces left behind.
 __device__ __forceinline__ unsigned stage_mask(int stage, bool valid, double bound, double qx, double qy, double qz, int vx, int vy,
@@ -353,6 +342,9 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
     __shared__ double s_sum[8];
     __shared__ int s_flag[2];
     __shared__ volatile int s_ncls[2];  // a later pass's search: points of the heavy and the middle class
+    // thread 0's %globaltimer stamps of the pass (start, end of the certificate phase, end of its barrier): in shared memory, so
+    // that no register of the window loop is spent on them
+    __shared__ unsigned long long s_t[3];
 
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int quad = lane >> 2, sub = lane & 3;
@@ -378,14 +370,14 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
     __syncthreads();
     if (!PERSISTENT && s_ps.done) return;
 
-    unsigned long long n_probe = 0, n_cand = 0, n_line = 0;
     unsigned tbase = 0;  // first ticket of the current phase (identical in every warp of the grid)
     KR_PROF_DECL
 
     for (unsigned it = 0; !s_ps.done; ++it) {
 #pragma unroll
         for (int k = 0; k < 7; ++k) sm.acc[k][lane] = 0.0;
-        const unsigned long long t_iter0 = gtime_ns();
+        if (threadIdx.x == 0) s_t[0] = s_t[1] = s_t[2] = gtime_ns();
+        KR_WLOG_DO(const unsigned long long wl_it0 = gtime_ns();)
         KR_PROF_PASS(it)
         const double inv_vs = 1.0 / a.map.voxel_size;
         // tasks per batch: a batch's lines must fit the line buffer even if every voxel is full
@@ -395,7 +387,6 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
         // ticket beyond the range of a phase, so a phase of W windows consumes W + total_warps tickets).
         unsigned tk = 0;  // lane 0: the ticket drawn ahead of time (the atomic's round trip is off the critical path)
         int nsearch = num_windows;  // windows of the search phase of this pass
-        unsigned long long t_a1 = t_iter0, t_a2 = t_iter0;  // end of the certificate phase / of its barrier (thread 0)
 
         if (cache && it > 0u) {
             // ------------------------------------------------------------------------------------------------------------
@@ -496,11 +487,11 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                 pos = __shfl_sync(FULL, pos, max(cls, 0)) + (unsigned)__popc(need & ((1u << lane) - 1u));
                 if (cls >= 0) *class_entry(a, n, cls, pos) = (unsigned)i;
             }
-            KR_WLOG(1, t_iter0, gtime_ns(), 0, 0)
+            KR_WLOG(1, wl_it0, gtime_ns(), 0, 0)
             // every CTA of the grid has to be through phase A before the list is complete
             __syncthreads();
             if (threadIdx.x == 0) {
-                t_a1 = gtime_ns();
+                s_t[1] = gtime_ns();
                 __threadfence();
                 atomicAdd(&st->a_arrive, 1u);
                 const unsigned target = it * gridDim.x;
@@ -512,7 +503,7 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                         break;
                     }
                 }
-                t_a2 = gtime_ns();
+                s_t[2] = gtime_ns();
                 s_ncls[0] = (int)__ldcg(&st->cls_n[1][it]), s_ncls[1] = (int)__ldcg(&st->cls_n[2][it]);
             }
             __syncthreads();
@@ -608,13 +599,13 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                     }
                 }
             }
-            double seed2 = DBL_MAX, seed_d = 3.0e38;  // (squared) distance to the previous neighbour — an exact pruning bound —, if it applies
+            double seed_d = 3.0e38;  // distance to the previous neighbour — an exact pruning bound —, if it applies (< 1e38)
             {
                 double px = 0, py = 0, pz = 0;
                 if (valid) load_scan_point(a.scan, pi, px, py, pz);
                 if (indirect && valid) {
                     const double sd = (double)__ldcg(&a.nn_l[pi]);  // (the seed, left there by the certificate sweep)
-                    if (sd < 1.0e38) seed_d = sd, seed2 = sd * sd * (1.0 + 1e-6);
+                    if (sd < 1.0e38) seed_d = sd;
                 }
                 double qx, qy, qz;
                 query_rn(s_ps.q, s_ps.t, px, py, pz, qx, qy, qz);
@@ -625,8 +616,10 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                 sm.px[lane] = px, sm.py[lane] = py;
             }
             // the owner's running minimum lives in its lane's registers: d^2, the line that holds it, how many points that line has;
-            // the runner-up lines and `minpruned` (the cubes of the voxels that were skipped) feed the certificate of the next pass
-            double best = DBL_MAX, second = DBL_MAX, third = DBL_MAX, minpruned = DBL_MAX;  // three smallest LINE minima (+ skipped cubes)
+            // the runner-up line and `lo` feed the certificate of the next pass.  `lo` is the smallest line minimum that is neither
+            // `best` nor `second` (whatever either of them gives up goes into it) and the cubes of the voxels that were skipped: the
+            // certificate only needs the minimum of all of these, so one register holds it
+            double best = DBL_MAX, second = DBL_MAX, lo = DBL_MAX;
             unsigned bline = 0xFFFFFFFFu, bvalid = 0u;   // the line holding `best` ...
             unsigned sline = 0xFFFFFFFFu, svalid = 0u;   // ... and the one holding `second`
             __syncwarp();
@@ -645,15 +638,16 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                     // exact pruning bound: the best squared distance found so far, and never more than the gate — a neighbour at
                     // tau or beyond is rejected anyway (Registration.cpp:75), so voxels that can only hold such points are skipped
                     const double tau2 = s_ps.tau * s_ps.tau;
+                    const double seed2 = seed_d < 1.0e38 ? seed_d * seed_d * (1.0 + 1e-6) : DBL_MAX;
                     const double bsq = fmin(fmin(tau2, best), seed2);
                     const double bound = bsq * (1.0 + 1e-6) + 1e-10;
                     unsigned mask = stage_mask(stage, valid, bound, qq.x, qq.y, sm.qz[lane], sm.vx[lane], sm.vy[lane], sm.vz[lane],
-                                               a.map.voxel_size, minpruned);
+                                               a.map.voxel_size, lo);
                     if (stage == 0 && valid && seed_d < 1.0e38) {
-                        double mp = minpruned;
+                        double mp = lo;
                         const unsigned near = seeded_near_mask(seed_d, s_ps.tau, qq.x, qq.y, sm.qz[lane], sm.vx[lane], sm.vy[lane], sm.vz[lane],
                                                                a.map.voxel_size, mp);
-                        if (__popc(near) <= KR_MERGE_MAX) mask |= near, minpruned = mp, merged = true;  // (a loose bound keeps the staged way)
+                        if (__popc(near) <= KR_MERGE_MAX) mask |= near, lo = mp, merged = true;  // (a loose bound keeps the staged way)
                     }
                     mask &= ~donem;
                     donem |= mask;
@@ -743,7 +737,15 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                         if (lane >= d) incl += y;
                     }
                     const int ltot = __shfl_sync(FULL, incl, 31);
-                    if (a.collect_stats) n_probe += act ? 1 : 0, n_cand += cnt, n_line += nl;
+                    if (a.collect_stats) {  // option "stats": the batch's warp sums, one atomic per counter (no register held for them)
+                        int csum = cnt;
+#pragma unroll
+                        for (int d = 16; d > 0; d >>= 1) csum += __shfl_xor_sync(FULL, csum, d);
+                        const unsigned nprobe = (unsigned)__popc(__ballot_sync(FULL, act));
+                        if (lane == 0)
+                            atomicAdd(&st->stats[0], (unsigned long long)nprobe), atomicAdd(&st->stats[1], (unsigned long long)csum),
+                                atomicAdd(&st->stats[2], (unsigned long long)ltot);
+                    }
 
                     if ((!more || fill + ltot > KR_LCAP) && fill > 0) {
                         // ---------------------------------------------------- evaluate the buffered lines
@@ -788,15 +790,15 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                                     const double dl = sm.lmin[lb + u];
                                     if (closer(dl, best)) {
                                         const LineDesc ld = sm.ldesc[lb + u];
-                                        third = second;
+                                        lo = fmin(lo, second);
                                         second = best, sline = bline, svalid = bvalid;
                                         best = dl, bline = ld.gline, bvalid = ld.nvalid;
                                     } else if (dl < second) {
                                         const LineDesc ld = sm.ldesc[lb + u];
-                                        third = second;
+                                        lo = fmin(lo, second);
                                         second = dl, sline = ld.gline, svalid = ld.nvalid;
                                     } else {
-                                        third = fmin(third, dl);
+                                        lo = fmin(lo, dl);
                                     }
                                 }
                             }
@@ -884,7 +886,7 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                             else ru2 = fmin(ru2, de);
                         }
                     }
-                    const double lo2 = fmin(fmin(ru2, third), minpruned);
+                    const double lo2 = fmin(ru2, lo);
                     a.nn_g[pi] = have ? g0 + (unsigned)jw : 0xFFFFFFFFu;
                     a.nn_g2[pi] = g2;
                     a.nn_l[pi] = lo2 >= 1.0e60 ? 1.0e30f : __double2float_rz(sqrt(lo2) * (1.0 - 1e-7));
@@ -942,7 +944,6 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                 }
                 if (threadIdx.x == 0) st->ticket = 0, st->win_ctr = 0;
             }
-            if (a.collect_stats) stats_flush(st, n_probe, n_cand, n_line);
             return;
         }
 
@@ -1046,7 +1047,7 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
                 solve_and_update(&s_ps, s, blockIdx.x == 0 ? &st->result : nullptr, blockIdx.x == 0 ? a.init.iters_out : nullptr);
             }
             if (blockIdx.x == 0 && it < KICP_MAX_ITERATIONS) {
-                st->dbg[it][0] = (double)(t_a1 - t_iter0), st->dbg[it][1] = (double)(t_a2 - t_a1), st->dbg[it][2] = (double)(t_win - t_a2);
+                st->dbg[it][0] = (double)(s_t[1] - s_t[0]), st->dbg[it][1] = (double)(s_t[2] - s_t[1]), st->dbg[it][2] = (double)(t_win - s_t[2]);
                 st->dbg[it][3] = (double)(t_arr - t_win), st->dbg[it][4] = (double)(t_red - t_arr), st->dbg[it][5] = (double)(gtime_ns() - t_red);
             }
         }
@@ -1054,7 +1055,6 @@ __global__ void __launch_bounds__(KR_THREADS, KR_MINB) k_register(const KernelAr
     }
 
     if (PERSISTENT) {
-        if (a.collect_stats) stats_flush(st, n_probe, n_cand, n_line);
         KR_PROF_FLUSH
         __syncthreads();
         // the result block goes straight to the caller's page-locked host memory (no copy-engine operation after the kernel)

@@ -10,7 +10,7 @@ import kinematic_icp_b200 as kb
 from kinematic_icp_b200 import _capi
 from oracle import workloads as W
 
-KR_WARPS = 10
+KR_WARPS = 8
 cfg = int(sys.argv[1]) if len(sys.argv) > 1 else 4
 outdir = sys.argv[2] if len(sys.argv) > 2 else "."
 w = W.Workload(cfg)
