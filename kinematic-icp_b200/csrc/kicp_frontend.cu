@@ -519,7 +519,7 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
     int status = r.status;
     // a NaN pose (zero correspondences, which the reference does not defend against) is reported and leaves the map untouched
     if (one_sync) {
-        const int mst = kicp_map_finish_update(map, s.h_mapctr);
+        const int mst = kicp_map_finish_update(map, s.h_mapctr, false);
         if (mst != KICP_OK) status = mst;
     } else if (status == KICP_OK && counts[1] > 0) {
         status = kicp_map_update_pose_device(map, reinterpret_cast<const double *>(s.out2), counts[1], r.pose);

@@ -184,7 +184,8 @@ int kicp_map_update_pose_device(kicp_map *m, const double *d_xyz, int64_t n, con
 // the same with the point count and the pose still on the device (no read-back; kicp_map.cu)
 int kicp_map_update_pose_async(kicp_map *m, const double *d_xyz, int64_t n_max, const int *d_n, const kicp_reg_result *d_res,
                                uint32_t *h_counters);
-int kicp_map_finish_update(kicp_map *m, const uint32_t *h_counters);
+// the host mirrors from the counters an update copied back (`evict_only`: those of RemovePointsFarFromLocation alone)
+int kicp_map_finish_update(kicp_map *m, const uint32_t *ctr, bool evict_only);
 // device address of the result block the last enqueued registration on this context writes (kicp_register_api.cu)
 const kicp_reg_result *kicp_device_result(kicp_ctx *c);
 // defined in kicp_register.cu: enqueue one registration of n device-resident points on the context stream; the result

@@ -230,8 +230,10 @@ static uint32_t next_pow2(uint64_t v) {
     return (uint32_t)p;
 }
 
-// (Re)build the open-addressed table over the first `nslots` slots of the slab's table region (nslots <= slots_cap)
-static int map_rebuild_table(kicp_map *m, uint32_t nslots) {
+// (Re)build the open-addressed table over the first `nslots` slots of the slab's table region (nslots <= slots_cap) from the first
+// `nb` blocks.  `ctr` (the frame path): the counters of the update just enqueued, from which k_table_rebuild reads the block count;
+// nb is then its upper bound.
+static int map_rebuild_table(kicp_map *m, uint32_t nslots, uint32_t nb, const uint32_t *ctr = nullptr) {
     kicp_ctx *c = m->ctx;
     if (nslots > m->slots_cap) {
         kicp_set_error("voxel map: internal error, table larger than its slab region");
@@ -239,8 +241,8 @@ static int map_rebuild_table(kicp_map *m, uint32_t nslots) {
     }
     m->nslots = nslots;
     KICP_CUDA(cudaMemsetAsync(m->slots, 0xFF, (size_t)m->nslots * sizeof(int4), c->stream));
-    if (m->num_blocks) {
-        k_table_rebuild<<<(m->num_blocks + 255) / 256, 256, 0, c->stream>>>(m->slots, m->nslots - 1, m->blk, m->num_blocks);
+    if (nb) {
+        k_table_rebuild<<<(nb + 255) / 256, 256, 0, c->stream>>>(m->slots, m->nslots - 1, m->blk, nb, ctr);
         KICP_CHECK_LAUNCH(c);
     }
     return KICP_OK;
@@ -283,7 +285,7 @@ static int map_alloc_storage(kicp_map *m, uint32_t ncap) {
     m->d_keep = reinterpret_cast<uint32_t *>(slab + o_keep), m->d_new_id = reinterpret_cast<uint32_t *>(slab + o_id);
     m->slots = reinterpret_cast<int4 *>(slab + o_slots), m->slots_cap = slots_cap;
     // the table moved with the slab: rebuild it at its previous size (or the minimum for a new map)
-    return map_rebuild_table(m, std::max<uint32_t>(std::min(m->nslots, slots_cap), 1024u));
+    return map_rebuild_table(m, std::max<uint32_t>(std::min(m->nslots, slots_cap), 1024u), m->num_blocks);
 }
 
 // make room for `extra` more voxels (blocks) and keep the table load factor <= 0.25
@@ -298,7 +300,7 @@ static int map_reserve(kicp_map *m, uint64_t extra) {
         KICP_TRY(map_alloc_storage(m, (uint32_t)std::min<uint64_t>(grown, 1ull << 24)));
     }
     const uint32_t want_slots = std::max<uint32_t>(next_pow2(need * 4), 1024u);
-    if (want_slots > m->nslots) KICP_TRY(map_rebuild_table(m, want_slots));
+    if (want_slots > m->nslots) KICP_TRY(map_rebuild_table(m, want_slots, m->num_blocks));
     return KICP_OK;
 }
 
@@ -391,43 +393,91 @@ extern "C" int kicp_map_num_voxels(kicp_map *m, int64_t *n) {
     return KICP_OK;
 }
 
-// `src_on_device`: xyz is a device pointer (packed doubles) that stays valid until the stream drains
-static int map_add_points_impl(kicp_map *m, const double *xyz, int64_t n, const double *pose7, bool src_on_device = false) {
-    if (!m || n < 0 || (n > 0 && !xyz)) return KICP_ERR_INVALID;
-    if (n == 0) return KICP_OK;
+// The host mirrors from the counter words of an update, once the stream has drained.  The kernels define the words
+// (kicp_map_kernels.cuh): [0] blocks after the insert, [2] overflow, [3] points inserted, [4] blocks evicted, [5] points evicted by
+// the frame path's k_mark_far.  A synchronous eviction (`evict_only`) has counters of its own, and its k_mark_far counts the points
+// evicted in word 3.
+int kicp_map_finish_update(kicp_map *m, const uint32_t *ctr, bool evict_only) {
+    if (!m || !ctr) return KICP_ERR_INVALID;
+    // cannot happen: map_reserve makes room for one new block per point before every insert
+    if (ctr[2]) {
+        kicp_set_error("voxel map: block storage overflow during AddPoints");
+        return KICP_ERR_CAPACITY;
+    }
+    const int64_t added = evict_only ? 0 : ctr[3], removed = ctr[evict_only ? 3 : 5];
+    m->num_blocks = (evict_only ? m->num_blocks : ctr[0]) - ctr[4];
+    m->num_points += added - removed;
+    return KICP_OK;
+}
+
+// AddPoints of the `n` points at `xyz` (a host array, or with `xyz_on_device` packed doubles in HBM that stay valid until the stream
+// drains), enqueued on the context stream.  The points are transformed by the pose first when there is one: `pose7` from the host,
+// or on the frame path the pose of `d_res`, the result block of the registration enqueued before, with the point count `d_n` (<= n)
+// also read on the device.
+static int map_insert(kicp_map *m, const double *xyz, bool xyz_on_device, int64_t n, const double *pose7, const int *d_n,
+                      const kicp_reg_result *d_res) {
     kicp_ctx *c = m->ctx;
     KICP_CUDA(cudaSetDevice(c->device));
     KICP_TRY(map_reserve_input(m, n));
-    KICP_TRY(map_reserve(m, (uint64_t)n));  // worst case: every point opens a new voxel
-    const double *d_src = xyz;
-    if (!src_on_device) {
+    KICP_TRY(map_reserve(m, (uint64_t)n));  // worst case: every point opens a new voxel (grows — and synchronises — rarely)
+    if (!xyz_on_device) {
         KICP_CUDA(cudaMemcpyAsync(m->d_in, xyz, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-        d_src = m->d_in;
+        xyz = m->d_in;
     }
-    uint32_t init[8] = {m->num_blocks, 0, 0, 0, 0, 0, 0, 0};
+    const uint32_t init[8] = {m->num_blocks, 0, 0, 0, 0, 0, 0, 0};
     KICP_CUDA(cudaMemcpyAsync(m->d_counters, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
     MapRW rw{m->slots, m->nslots - 1, m->blk, m->pts, m->pend_head, m->blocks_cap, (int)m->cap, m->voxel_size};
     Pose pose{0, 0, 0, 1, 0, 0, 0};
     if (pose7) pose = Pose{pose7[0], pose7[1], pose7[2], pose7[3], pose7[4], pose7[5], pose7[6]};
-    const int threads = 256;
-    k_add_find_or_create<<<(unsigned)((n + threads - 1) / threads), threads, 0, c->stream>>>(
-        rw, d_src, n, pose7 ? 1 : 0, pose, m->d_xyz_t, m->d_next, m->d_counters, m->d_touched);
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    k_add_find_or_create<<<grid, 256, 0, c->stream>>>(rw, xyz, n, pose7 || d_res ? 1 : 0, pose, m->d_xyz_t, m->d_next, m->d_counters,
+                                                     m->d_touched, d_n, d_res);
     KICP_CHECK_LAUNCH(c);
     // KISS AddPoints: map_resolution = sqrt(voxel_size^2 / max_points_per_voxel)
     const double map_resolution = std::sqrt(m->voxel_size * m->voxel_size / (double)m->cap);
-    k_add_commit<<<(unsigned)((n + threads - 1) / threads), threads, 0, c->stream>>>(rw, m->d_xyz_t, m->d_next, m->d_counters,
-                                                                                 m->d_touched, map_resolution);
+    k_add_commit<<<grid, 256, 0, c->stream>>>(rw, m->d_xyz_t, m->d_next, m->d_counters, m->d_touched, map_resolution);
+    KICP_CHECK_LAUNCH(c);
+    return KICP_OK;
+}
+
+// RemovePointsFarFromLocation over the first `nb` blocks: k_mark_far flags the survivors, which are compacted (order kept) into the
+// spare arrays; those swap with the live ones and the table is rebuilt.  Synchronous (`d_res` null): the eviction zeroes the
+// counters, reads them back after k_mark_far and compacts only when a voxel died.  Frame path: the origin and the registration's
+// status are read from `d_res` on the device (`origin` is unused) and the block count from the insert's counters (nb is its upper
+// bound).  Nothing is read back and the compaction always runs — a moving sensor evicts voxels on practically every frame anyway,
+// and the host cannot know.
+static int map_evict(kicp_map *m, const double origin[3], const kicp_reg_result *d_res, uint32_t nb) {
+    kicp_ctx *c = m->ctx;
+    const uint32_t init[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (!d_res) KICP_CUDA(cudaMemcpyAsync(m->d_counters, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
+    k_mark_far<<<(nb + 255) / 256, 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, nb, origin[0], origin[1], origin[2],
+                                                       m->max_distance * m->max_distance, m->d_keep, m->d_counters, d_res);
     KICP_CHECK_LAUNCH(c);
     uint32_t res[8];
-    KICP_CUDA(cudaMemcpyAsync(res, m->d_counters, sizeof(res), cudaMemcpyDeviceToHost, c->stream));
-    KICP_CUDA(cudaStreamSynchronize(c->stream));
-    if (res[2]) {
-        kicp_set_error("voxel map: block storage overflow during AddPoints");
-        return KICP_ERR_CAPACITY;
+    if (!d_res) {
+        KICP_CUDA(cudaMemcpyAsync(res, m->d_counters, sizeof(res), cudaMemcpyDeviceToHost, c->stream));
+        KICP_CUDA(cudaStreamSynchronize(c->stream));
+        if (res[4] == 0) return KICP_OK;
     }
-    m->num_blocks = res[0];
-    m->num_points += res[3];
-    return KICP_OK;
+    KICP_TRY(enqueue_exclusive_sum(c, m->d_keep, m->d_new_id, nb));
+    k_compact_blocks<<<(unsigned)(((uint64_t)nb * 32 + 255) / 256), 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, nb, m->d_keep,
+                                                                                       m->d_new_id, m->blk_spare, m->pts_spare);
+    KICP_CHECK_LAUNCH(c);
+    std::swap(m->blk, m->blk_spare);
+    std::swap(m->pts, m->pts_spare);
+    if (!d_res) KICP_TRY(kicp_map_finish_update(m, res, true));
+    return map_rebuild_table(m, m->nslots, d_res ? nb : m->num_blocks, d_res ? m->d_counters : nullptr);  // after the compaction
+}
+
+// AddPoints with the count and the pose on the host: one synchronisation, after which the host mirrors are current
+static int map_add_points_impl(kicp_map *m, const double *xyz, int64_t n, const double *pose7, bool xyz_on_device = false) {
+    if (!m || n < 0 || (n > 0 && !xyz)) return KICP_ERR_INVALID;
+    if (n == 0) return KICP_OK;
+    KICP_TRY(map_insert(m, xyz, xyz_on_device, n, pose7, nullptr, nullptr));
+    uint32_t res[8];
+    KICP_CUDA(cudaMemcpyAsync(res, m->d_counters, sizeof(res), cudaMemcpyDeviceToHost, m->ctx->stream));
+    KICP_CUDA(cudaStreamSynchronize(m->ctx->stream));
+    return kicp_map_finish_update(m, res, false);
 }
 
 extern "C" int kicp_map_add_points(kicp_map *m, const double *xyz, int64_t n) { return map_add_points_impl(m, xyz, n, nullptr); }
@@ -435,32 +485,8 @@ extern "C" int kicp_map_add_points(kicp_map *m, const double *xyz, int64_t n) { 
 extern "C" int kicp_map_remove_far(kicp_map *m, const double origin[3]) {
     if (!m || !origin) return KICP_ERR_INVALID;
     if (m->num_blocks == 0) return KICP_OK;
-    kicp_ctx *c = m->ctx;
-    KICP_CUDA(cudaSetDevice(c->device));
-    uint32_t *keep = m->d_keep, *new_id = m->d_new_id;
-    uint32_t init[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    KICP_CUDA(cudaMemcpyAsync(m->d_counters, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
-    k_mark_far<<<(m->num_blocks + 255) / 256, 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, m->num_blocks, origin[0], origin[1],
-                                                                  origin[2], m->max_distance * m->max_distance, keep,
-                                                                  m->d_counters);
-    KICP_CHECK_LAUNCH(c);
-    uint32_t res[8];
-    KICP_CUDA(cudaMemcpyAsync(res, m->d_counters, sizeof(res), cudaMemcpyDeviceToHost, c->stream));
-    KICP_CUDA(cudaStreamSynchronize(c->stream));
-    if (res[4] > 0) {
-        // compact surviving blocks (order preserved) into the spare arrays, swap, and rebuild the table
-        const uint32_t survivors = m->num_blocks - res[4];
-        KICP_TRY(enqueue_exclusive_sum(c, keep, new_id, m->num_blocks));
-        k_compact_blocks<<<(unsigned)(((uint64_t)m->num_blocks * 32 + 255) / 256), 256, 0, c->stream>>>(
-            m->blk, m->pts, (int)m->cap, m->num_blocks, keep, new_id, m->blk_spare, m->pts_spare);
-        KICP_CHECK_LAUNCH(c);
-        std::swap(m->blk, m->blk_spare);
-        std::swap(m->pts, m->pts_spare);
-        m->num_blocks = survivors;
-        m->num_points -= res[3];
-        KICP_TRY(map_rebuild_table(m, m->nslots));  // stream-ordered after the compaction
-    }
-    return KICP_OK;
+    KICP_CUDA(cudaSetDevice(m->ctx->device));
+    return map_evict(m, origin, nullptr, m->num_blocks);
 }
 
 extern "C" int kicp_map_update(kicp_map *m, const double *xyz, int64_t n, const double origin[3]) {
@@ -479,54 +505,17 @@ int kicp_map_update_pose_device(kicp_map *m, const double *d_xyz, int64_t n, con
 }
 
 // local_map_.Update(frame, pose) (KinematicICP.cpp:79) for a frame whose point count (`d_n` <= n_max) and pose (`d_res`) are
-// still being computed on the stream: everything is enqueued, nothing is read back.  The eviction always compacts (into the spare
-// arrays, then the arrays swap) — a moving sensor evicts voxels on practically every frame anyway, and the host cannot know.
-// The counters are copied to `h_counters` (pinned, 8 words); after the caller's end-of-frame synchronisation,
-// kicp_map_finish_update() brings the host mirrors up to date.
+// still being computed on the stream: everything is enqueued, nothing is read back.  The counters are copied to `h_counters`
+// (pinned, 8 words); after the caller's end-of-frame synchronisation, kicp_map_finish_update() brings the host mirrors up to date.
 int kicp_map_update_pose_async(kicp_map *m, const double *d_xyz, int64_t n_max, const int *d_n, const kicp_reg_result *d_res,
                                uint32_t *h_counters) {
     if (!m || n_max <= 0 || !d_xyz || !d_n || !d_res || !h_counters) return KICP_ERR_INVALID;
-    kicp_ctx *c = m->ctx;
-    KICP_CUDA(cudaSetDevice(c->device));
-    KICP_TRY(map_reserve_input(m, n_max));
-    KICP_TRY(map_reserve(m, (uint64_t)n_max));  // worst case: every point opens a new voxel (grows — and synchronises — rarely)
-    const uint32_t init[8] = {m->num_blocks, 0, 0, 0, 0, 0, 0, 0};
-    KICP_CUDA(cudaMemcpyAsync(m->d_counters, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
-    MapRW rw{m->slots, m->nslots - 1, m->blk, m->pts, m->pend_head, m->blocks_cap, (int)m->cap, m->voxel_size};
-    const int threads = 256;
-    const unsigned pgrid = (unsigned)((n_max + threads - 1) / threads);
-    k_add_find_or_create<<<pgrid, threads, 0, c->stream>>>(rw, d_xyz, n_max, 1, Pose{0, 0, 0, 1, 0, 0, 0}, m->d_xyz_t, m->d_next, m->d_counters,
-                                                        m->d_touched, d_n, d_res);
-    KICP_CHECK_LAUNCH(c);
-    const double map_resolution = std::sqrt(m->voxel_size * m->voxel_size / (double)m->cap);
-    k_add_commit<<<pgrid, threads, 0, c->stream>>>(rw, m->d_xyz_t, m->d_next, m->d_counters, m->d_touched, map_resolution);
-    KICP_CHECK_LAUNCH(c);
+    KICP_TRY(map_insert(m, d_xyz, true, n_max, nullptr, d_n, d_res));
     // RemovePointsFarFromLocation(pose.translation()) over the blocks that exist now: at most ub
     const uint32_t ub = (uint32_t)std::min<uint64_t>((uint64_t)m->num_blocks + (uint64_t)n_max, m->blocks_cap);
-    k_mark_far<<<(ub + 255) / 256, 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, ub, 0.0, 0.0, 0.0, m->max_distance * m->max_distance,
-                                                     m->d_keep, m->d_counters, d_res);
-    KICP_CHECK_LAUNCH(c);
-    KICP_TRY(enqueue_exclusive_sum(c, m->d_keep, m->d_new_id, ub));
-    k_compact_blocks<<<(unsigned)(((uint64_t)ub * 32 + 255) / 256), 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, ub, m->d_keep,
-                                                                                       m->d_new_id, m->blk_spare, m->pts_spare);
-    KICP_CHECK_LAUNCH(c);
-    std::swap(m->blk, m->blk_spare);
-    std::swap(m->pts, m->pts_spare);
-    KICP_CUDA(cudaMemsetAsync(m->slots, 0xFF, (size_t)m->nslots * sizeof(int4), c->stream));
-    k_table_rebuild<<<(ub + 255) / 256, 256, 0, c->stream>>>(m->slots, m->nslots - 1, m->blk, ub, m->d_counters);
-    KICP_CHECK_LAUNCH(c);
-    KICP_CUDA(cudaMemcpyAsync(h_counters, m->d_counters, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
-    return KICP_OK;
-}
-// after the stream has drained: host mirrors from the counters of kicp_map_update_pose_async
-int kicp_map_finish_update(kicp_map *m, const uint32_t *h_counters) {
-    if (!m || !h_counters) return KICP_ERR_INVALID;
-    m->num_blocks = h_counters[0] - h_counters[4];
-    m->num_points += (int64_t)h_counters[3] - (int64_t)h_counters[5];
-    if (h_counters[2]) {
-        kicp_set_error("voxel map: block storage overflow during AddPoints");
-        return KICP_ERR_CAPACITY;
-    }
+    const double unused[3] = {0.0, 0.0, 0.0};
+    KICP_TRY(map_evict(m, unused, d_res, ub));
+    KICP_CUDA(cudaMemcpyAsync(h_counters, m->d_counters, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, m->ctx->stream));
     return KICP_OK;
 }
 
@@ -561,7 +550,8 @@ static int map_download_packed(kicp_map *m, T *out_xyz, std::vector<int4> *hdr) 
     return KICP_OK;
 }
 
-extern "C" int kicp_map_pointcloud(kicp_map *m, double *out_xyz, int64_t cap, int64_t *n) {
+template <class T>
+static int map_pointcloud(kicp_map *m, T *out_xyz, int64_t cap, int64_t *n) {
     if (!m || !n) return KICP_ERR_INVALID;
     *n = m->num_points;
     if (m->num_points > cap) return KICP_ERR_CAPACITY;
@@ -570,16 +560,11 @@ extern "C" int kicp_map_pointcloud(kicp_map *m, double *out_xyz, int64_t cap, in
     return map_download_packed(m, out_xyz, nullptr);
 }
 
+extern "C" int kicp_map_pointcloud(kicp_map *m, double *out_xyz, int64_t cap, int64_t *n) { return map_pointcloud(m, out_xyz, cap, n); }
+
 // Pointcloud() as the float32 records EigenToPointCloud2 builds from it (RosUtils.cpp:41-63): the same order, half the bytes, and
 // the narrowing done on the device by the reference's x86-64 rule (to_f32_x86)
-extern "C" int kicp_map_pointcloud_f32(kicp_map *m, float *out_xyz, int64_t cap, int64_t *n) {
-    if (!m || !n) return KICP_ERR_INVALID;
-    *n = m->num_points;
-    if (m->num_points > cap) return KICP_ERR_CAPACITY;
-    if (m->num_points == 0) return KICP_OK;
-    if (!out_xyz) return KICP_ERR_INVALID;
-    return map_download_packed(m, out_xyz, nullptr);
-}
+extern "C" int kicp_map_pointcloud_f32(kicp_map *m, float *out_xyz, int64_t cap, int64_t *n) { return map_pointcloud(m, out_xyz, cap, n); }
 
 // ------------------------------------------------------------------------------------------- live local-map cloud
 #include "kicp_map_live_kernels.cuh"  // struct LiveArgs and the k_live_* kernels
@@ -789,7 +774,7 @@ extern "C" int kicp_map_load_voxels(kicp_map *m, const int32_t *keys, const int3
     KICP_CHECK_LAUNCH(c);
     m->num_blocks = (uint32_t)num_voxels;
     m->num_points = total;
-    int st = map_rebuild_table(m, m->nslots);
+    int st = map_rebuild_table(m, m->nslots, m->num_blocks);
     cudaError_t e = cudaStreamSynchronize(c->stream);
     cudaFree(d_keys), cudaFree(d_counts), cudaFree(d_off), cudaFree(d_pts);
     if (st != KICP_OK) return st;
