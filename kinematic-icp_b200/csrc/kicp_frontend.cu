@@ -489,14 +489,14 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
     s.timing[0] = ms_since();  // upload + front end (ingest, de-skew, filter, transform, both down-samples)
     // (in the single-synchronisation order the counts are still 0 and the caller's buffers hold n points)
     if ((a.out_frame && counts[0] > a.cap_frame) || (a.out_source && counts[2] > a.cap_source)) return KICP_ERR_CAPACITY;
-    if (one_sync) {
-        if (stage || stage32) KICP_CUDA(cudaEventRecord(s.ev_front, c->stream));
-        c->reg_n_hint = s.last_source > 0 ? s.last_source + s.last_source / 4 + 256 : 0;  // the grid is planned from the previous source
-    }
-    // registration of the source against the local map, enqueued first so that the staging copies overlap it
+    if (one_sync && (stage || stage32)) KICP_CUDA(cudaEventRecord(s.ev_front, c->stream));
+    // registration of the source against the local map, enqueued first so that the staging copies overlap it; in the
+    // single-synchronisation order its grid is planned from the previous source
     const int64_t reg_n = one_sync ? n : counts[2];
+    const int64_t reg_hint = one_sync && s.last_source > 0 ? s.last_source + s.last_source / 4 + 256 : 0;
     KICP_TRY(kicp_enqueue_registration_device(map, reg_n ? reinterpret_cast<const double *>(s.out3) : nullptr, reg_n,
-                                              one_sync ? s.d_count + 2 : nullptr, a.last_pose, a.relative_odometry, a.tau, &fp->reg));
+                                              one_sync ? s.d_count + 2 : nullptr, a.last_pose, a.relative_odometry, a.tau, &fp->reg,
+                                              reg_hint));
     s.timing[1] = ms_since();  // + registration enqueued
     // the two clouds go to pinned staging on the copy stream while the registration runs; in the single-synchronisation order the
     // frame is copied for n points and the source for the previous frame's twofold (the rest follows below)

@@ -50,47 +50,26 @@ struct kicp_scan_args {
     uint32_t launch;
 };
 
+struct RegState;  // device-side state of one registration (kicp_register.cu)
+
 struct kicp_ctx {
     int device = 0;
     int sm_count = 132;
     cudaStream_t stream = nullptr;
     int64_t launches = 0;
-    // registration scratch
-    struct RegState *d_state = nullptr;
-    double *d_partials = nullptr;  // per-CTA partial sums of the registration kernel [2][grid][8]
-    int pruned_ctas_per_sm = 1;      // resident CTAs per SM of k_register<false> (occupancy query)
-    int persistent_ctas_per_sm = 1;  // ... of k_register<true>
+    // registration options (kicp_ctx_set_option)
     int ctas_per_sm_cap = 0;         // option "ctas_per_sm": 0 = use the occupancy limit
     int persistent = 1;     // 1 = all IRLS iterations inside one cooperative launch, 0 = one launch per iteration
     int collect_stats = 0;  // option "stats": count probes / candidate points / lines on the device
     int spin_timeout_ms = 20000;  // bound of every device-side wait (upload flags, peers of the fused exchange)
-    // nearest-neighbour cache of the persistent kernel (one entry per scan point, carried from pass to pass)
-    unsigned int *d_nn_g = nullptr, *d_nn_g2 = nullptr, *d_todo = nullptr, *d_todo2 = nullptr;
-    float *d_nn_l = nullptr;
-    int64_t nn_cap = 0;
     int nn_cache = 1;  // option "nn_cache"
     int frame_sync = 0;       // option "frame_sync": 1 = kicp_register_frame reads the survivor counts back mid-frame (legacy order)
     int downsample_order = 0;  // option "downsample_order": 1 = VoxelDownsample emits the robin_map's bucket order (kicp_frontend.cu)
-    int64_t reg_n_hint = 0;   // expected point count of the next registration whose exact count lives on the device (0 = none)
-    kicp_scan *upload_scan = nullptr;  // staging scan used by the host-pointer entry points
-    // chunked upload overlapped with the first IRLS iteration (host-pointer entry points, persistent kernel)
-    cudaStream_t copy_stream = nullptr;
-    uint32_t *d_chunk_flags = nullptr;   // [KICP_UPLOAD_CHUNKS] raised (to the upload sequence number) chunk by chunk
-    uint32_t *h_chunk_tags = nullptr;    // pinned source of the flag copies
-    uint32_t upload_seq = 0;
     int overlap_upload = 1;
+    // the registration's device state, neighbour cache, upload flags and profiling records (kicp_register_api.cu owns the type)
+    struct RegScratch *reg = nullptr;
+    cudaStream_t copy_stream = nullptr;   // copies that overlap the registration (the chunked frame upload, the staged clouds)
     kicp_reg_result *h_result = nullptr;  // pinned bounce buffer for synchronous calls
-    // profiling (kicp_ctx_profile_begin/end): event pairs per registration
-    bool profiling = false;
-    struct ProfReg {
-        cudaEvent_t prep0, prep1;
-        std::vector<cudaEvent_t> it;  // 2 per association launch
-        bool persistent = false;      // one launch covers every iteration
-        int32_t *d_iters;             // device word receiving the registration's iteration count
-    };
-    std::vector<ProfReg> prof;
-    int32_t *d_prof_iters = nullptr;
-    int64_t prof_cap = 0;
     // state of the single-pass scans (kicp_scan.cuh; stream-ordered, shared by the front end and the maps of this context)
     unsigned long long *d_scan_status = nullptr;
     unsigned int *d_scan_ticket = nullptr;
@@ -188,10 +167,14 @@ int kicp_map_update_pose_async(kicp_map *m, const double *d_xyz, int64_t n_max, 
 int kicp_map_finish_update(kicp_map *m, const uint32_t *ctr, bool evict_only);
 // device address of the result block the last enqueued registration on this context writes (kicp_register_api.cu)
 const kicp_reg_result *kicp_device_result(kicp_ctx *c);
-// defined in kicp_register.cu: enqueue one registration of n device-resident points on the context stream; the result
+// defined in kicp_register_api.cu: enqueue one registration of n device-resident points on the context stream; the result
 // lands in ctx->h_result (pinned) once the stream has drained
-// (`d_n`, optional: device-resident point count written earlier on the same stream; n_max is then the upper bound)
+// (`d_n`, optional: device-resident point count written earlier on the same stream; n_max is then the upper bound, and the
+// grid is planned for `n_hint` points, the count the producer expects, when that is smaller; 0 = no hint)
 int kicp_enqueue_registration_device(kicp_map *m, const double *d_xyz, int64_t n_max, const int *d_n, const double last[7],
-                                     const double odom[7], double tau, const kicp_reg_params *p);
+                                     const double odom[7], double tau, const kicp_reg_params *p, int64_t n_hint);
+// creates / frees the registration's scratch (kicp_ctx::reg) with the context (kicp_register_api.cu)
+int kicp_reg_scratch_create(kicp_ctx *c);
+void kicp_reg_scratch_free(kicp_ctx *c);
 // defined in kicp_comm.cu
 int kicp_comm_allreduce8(kicp_ctx *ctx, double *d_buf);

@@ -58,9 +58,7 @@ extern "C" int kicp_ctx_create(int device, kicp_ctx **out) {
     KICP_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     KICP_CUDA(cudaMallocHost(&c->h_result, sizeof(kicp_reg_result)));
     KICP_CUDA(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-    KICP_CUDA(cudaMalloc(&c->d_chunk_flags, KICP_UPLOAD_CHUNKS * sizeof(uint32_t)));
-    KICP_CUDA(cudaMemset(c->d_chunk_flags, 0, KICP_UPLOAD_CHUNKS * sizeof(uint32_t)));
-    KICP_CUDA(cudaMallocHost(&c->h_chunk_tags, KICP_UPLOAD_CHUNKS * sizeof(uint32_t)));
+    KICP_TRY(kicp_reg_scratch_create(c));
     if (const char *e = getenv("KICP_OVERLAP_UPLOAD")) c->overlap_upload = atoi(e) ? 1 : 0;
     if (const char *e = getenv("KICP_PERSISTENT")) c->persistent = atoi(e) ? 1 : 0;
     if (const char *e = getenv("KICP_CTAS_PER_SM")) c->ctas_per_sm_cap = std::min(16, std::max(0, atoi(e)));
@@ -162,20 +160,10 @@ extern "C" int kicp_ctx_destroy(kicp_ctx *ctx) {
     cudaStreamSynchronize(ctx->stream);
     kicp_comm_destroy(ctx);
     if (ctx->frontend_free) ctx->frontend_free(ctx);
-    if (ctx->upload_scan) kicp_scan_destroy(ctx->upload_scan);
-    cudaFree(ctx->d_state);
-    cudaFree(ctx->d_partials);
-    cudaFree(ctx->d_nn_g);
-    cudaFree(ctx->d_nn_g2);
-    cudaFree(ctx->d_nn_l);
-    cudaFree(ctx->d_todo);
-    cudaFree(ctx->d_todo2);
-    cudaFree(ctx->d_prof_iters);
+    kicp_reg_scratch_free(ctx);
     cudaFree(ctx->d_scan_status);
     cudaFree(ctx->d_scan_ticket);
     cudaFreeHost(ctx->h_result);
-    cudaFreeHost(ctx->h_chunk_tags);
-    cudaFree(ctx->d_chunk_flags);
     if (ctx->copy_stream) cudaStreamSynchronize(ctx->copy_stream), cudaStreamDestroy(ctx->copy_stream);
     cudaStreamDestroy(ctx->stream);
     delete ctx;
