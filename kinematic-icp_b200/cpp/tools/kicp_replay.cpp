@@ -17,10 +17,10 @@
 // and is replayed as the online node runs a frame: KinematicICP::StageFrame (the stamps decoded on the device, the sweep interval
 // back to the host), then RegisterStagedFrame.  --host-stamps replays it the host-decoding way instead: extract_timestamps +
 // process_timestamps + RegisterFrame.  Both write the same poses.
-// --device-input (KSEQ2, staged) replays a drive whose records a GPU producer left in device memory: every frame's records are copied
+// --device-input (KSEQ2 and KSEQ3, staged) replays a drive whose records a GPU producer left in device memory: every frame's records are copied
 // to device memory once, before the repetitions, and each frame is staged from there with KinematicICP::StageDeviceFrame, then
 // registered with RegisterStagedFrame as above.  Same poses again.  Not with --host-stamps or --pageable.
-// --publish (KSEQ2, staged) also builds, for every frame, the three clouds an online node publishes when it has subscribers
+// --publish (KSEQ2 and KSEQ3, staged) also builds, for every frame, the three clouds an online node publishes when it has subscribers
 // (LidarOdometryServer::PublishClouds, LidarOdometryServer.cpp:240-263: frame, keypoints, local map, each as EigenToPointCloud2's
 // float32 records): `host` the reference's way, RegisterStagedFrame + LocalMap() + the narrowing loop of EigenToPointCloud2
 // (RosUtils.cpp:41-63) restated below; `device` with RegisterStagedFramePointCloud2 + LocalMapPointCloud2, narrowed on the device;
@@ -32,6 +32,31 @@
 // may differ from run to run while its content does not.  The hashing is host work inside the timed loop: time without it.
 // --downsample-order 1 sets the default context's option "downsample_order" (kicp.h): both down-samples of every frame emit the
 // KISS-ICP robin_map order instead of the order of first occurrence (as KICP_DOWNSAMPLE_ORDER does for any facade program).
+//
+// Version 3, magic "KSEQ3\0\0\0", carries several message streams ("slots", 1..KICP_MAX_SENSORS: PointCloud2 records or 2D LaserScans,
+// each with its extrinsic) and the wheel odometry either as one relative motion or as poses sampled during the sweep:
+//   char magic[8]; int32 n_frames; int32 n_slots; double start_pose[7];
+//   per slot:  int32 kind (0 = PointCloud2 records, 1 = LaserScan); int32 stamps_relative; double lidar_to_base[7]
+//   per frame: double relative_odometry[7]; int32 n_samples; int32 reserved;
+//              n_samples x { double stamp; double pose[7] }   (the base pose in the odometry frame, on the odometry clock)
+//              per slot, in slot order, one message (it may be empty):
+//                kind 0: int32 n_points, point_step, offset_x, offset_y, offset_z, stamp_datatype, stamp_offset, reserved;
+//                        double header_stamp; uint8 records[n_points * point_step]          (the fields as in version 2)
+//                kind 1: int32 n_beams, reserved; double header_stamp;
+//                        float angle_min, angle_max, angle_increment, time_increment, range_min, range_max; float ranges[n_beams]
+// A records slot with stamps_relative 0 has absolute stamps (time_offset 0), with 1 stamps relative to its header (an Ouster `t`,
+// time_offset header_stamp); a LaserScan's offset is always its header stamp (kicp::SensorFrame).  Two slots may share an extrinsic
+// (two scans of a 25 Hz scanner against one 10 Hz sweep).  A frame is replayed as an online node runs one: one slot through
+// StageFrame / StageLaserScan (StageDevice* with --device-input) and RegisterStagedFrame, so that a one-slot drive is bit for bit the
+// version-2 drive of the same records; several through StageSensors and RegisterStagedSensors with the slots' extrinsics.
+// relative_odometry is T(begin)^-1 T(end) over the frame's sweep and keeps its role in the motion model and the threshold; n_samples 0
+// de-skews with it as one motion, otherwise the frame is de-skewed along the samples (the overloads taking kicp::OdometrySample), which
+// must cover the sweep the staging call returns (kicp/deskew_segments.hpp); a frame whose samples do not is an error.  The first sweep
+// begins at the earliest header stamp of the first frame, where the online node starts (LidarOdometryServer.cpp:182), and each TUM
+// line carries the end of its frame's sweep (offline_node.cpp:143-145), where versions 1 and 2 write the header stamp.  The file is
+// validated as a whole before the replay starts (kicp/kseq.hpp).  --host-stamps does not apply (there is no host-stamp call for
+// several sensors); the JSON line adds the slot kinds and the odometry samples per frame.
+//
 // Prints one JSON line with the frame rate; exits non-zero on any error (no CUDA
 // device included: there is no CPU fallback).
 #include <algorithm>
@@ -50,6 +75,7 @@
 #include <cuda_runtime.h>
 
 #include "kicp/facade_pipeline.hpp"
+#include "kicp/kseq.hpp"
 #include "kicp/runtime.hpp"
 #include "kicp/tum.hpp"
 
@@ -112,6 +138,69 @@ template <class T>
 void read_exact(std::FILE *f, T *dst, size_t count, const char *what) {
     if (std::fread(dst, sizeof(T), count, f) != count) throw std::runtime_error(std::string("truncated .kseq file while reading ") + what);
 }
+
+// a version-1 or version-2 drive: the frames into buffers of host_alloc; returns true for version 2
+bool read_kseq12(const char *path, bool pinned, double l2b[7], double start[7], std::vector<Frame> &frames, int64_t &total_points) {
+    std::FILE *f = std::fopen(path, "rb");
+    if (!f) throw std::runtime_error(std::string("cannot open ") + path);
+    char magic[8];
+    read_exact(f, magic, 8, "the header");
+    const bool v2 = std::memcmp(magic, "KSEQ2\0\0\0", 8) == 0;
+    if (!v2 && std::memcmp(magic, "KSEQ1\0\0\0", 8) != 0) throw std::runtime_error("not a .kseq file (bad magic)");
+    int32_t n_frames = 0, reserved = 0;
+    read_exact(f, &n_frames, 1, "the header"), read_exact(f, &reserved, 1, "the header");
+    read_exact(f, l2b, 7, "lidar_to_base"), read_exact(f, start, 7, "the start pose");
+    if (n_frames < 0 || n_frames > (1 << 24)) throw std::runtime_error("implausible frame count");
+    frames.resize((size_t)n_frames);
+    for (auto &fr : frames) {
+        if (v2) {
+            int32_t h[8];  // n, point_step, offset_x, offset_y, offset_z, stamp_datatype, stamp_offset, reserved
+            read_exact(f, h, 8, "a frame header");
+            read_exact(f, &fr.header_stamp, 1, "a frame header"), read_exact(f, fr.odom, 7, "a frame header");
+            if (h[0] < 0 || h[1] <= 0) throw std::runtime_error("bad point count or point_step");
+            fr.n = h[0];
+            const size_t bytes = (size_t)h[0] * (size_t)h[1];
+            uint8_t *raw = static_cast<uint8_t *>(host_alloc(bytes, pinned));
+            read_exact(f, raw, bytes, "records");
+            fr.msg.data = raw, fr.msg.width = (uint32_t)h[0], fr.msg.height = 1, fr.msg.point_step = (uint32_t)h[1];
+            fr.msg.fields = {{"x", (uint32_t)h[2], kicp::PF_FLOAT32, 1}, {"y", (uint32_t)h[3], kicp::PF_FLOAT32, 1},
+                             {"z", (uint32_t)h[4], kicp::PF_FLOAT32, 1}};
+            if (h[5] != 0) fr.msg.fields.push_back({"t", (uint32_t)h[6], (uint8_t)h[5], 1});
+            total_points += fr.n;
+            continue;
+        }
+        read_exact(f, &fr.n, 1, "a frame header"), read_exact(f, &fr.has_stamps, 1, "a frame header");
+        read_exact(f, &fr.header_stamp, 1, "a frame header"), read_exact(f, fr.odom, 7, "a frame header");
+        if (fr.n < 0) throw std::runtime_error("negative point count");
+        fr.xyz = static_cast<float *>(host_alloc((size_t)fr.n * 3 * sizeof(float), pinned));
+        read_exact(f, fr.xyz, (size_t)fr.n * 3, "points");
+        if (fr.has_stamps) {
+            fr.stamps = static_cast<double *>(host_alloc((size_t)fr.n * sizeof(double), pinned));
+            read_exact(f, fr.stamps, (size_t)fr.n, "stamps");
+        }
+        total_points += fr.n;
+    }
+    std::fclose(f);
+    return v2;
+}
+
+// the .kseq version of the file at `path` (kicp::kseq_version), 0 when it cannot be read
+int peek_version(const char *path) {
+    char magic[8];
+    std::FILE *f = std::fopen(path, "rb");
+    if (!f) return 0;
+    const bool ok = std::fread(magic, 1, 8, f) == 8;
+    std::fclose(f);
+    return ok ? kicp::kseq_version(magic) : 0;
+}
+
+// the points a staging call stages for a message: every record, or the beams projectLaser keeps (range_min <= r < range_max)
+int64_t staged_points(const kicp::SensorFrame &s) {
+    if (s.kind == kicp::SensorFrame::Kind::PointCloud2) return static_cast<int64_t>(s.cloud.num_points());
+    int64_t n = 0;
+    for (size_t i = 0; i < s.scan.n; ++i) n += s.scan.ranges[i] < s.scan.range_max && s.scan.ranges[i] >= s.scan.range_min;
+    return n;
+}
 }  // namespace
 
 int main(int argc, char **argv) {
@@ -166,69 +255,76 @@ int main(int argc, char **argv) {
         std::fprintf(stderr, "kicp_replay: --publish-digest needs --publish\n");
         return 2;
     }
+    const bool v3 = peek_version(argv[1]) == 3;  // other files: read (and refused) below
+    if (v3 && host_stamps) {
+        std::fprintf(stderr, "kicp_replay: --host-stamps replays a KSEQ2 drive; a KSEQ3 drive is always staged (there is no host-stamp "
+                     "call for several sensors)\n");
+        return 2;
+    }
     try {
         kicp::default_context();  // fails here, loudly, without a CUDA device
         if (downsample_order >= 0)
             kicp::check(kicp_ctx_set_option(kicp::default_context(), "downsample_order", downsample_order), "--downsample-order");
-        std::FILE *f = std::fopen(argv[1], "rb");
-        if (!f) throw std::runtime_error(std::string("cannot open ") + argv[1]);
-        char magic[8];
-        read_exact(f, magic, 8, "the header");
-        const bool v2 = std::memcmp(magic, "KSEQ2\0\0\0", 8) == 0;
-        if (!v2 && std::memcmp(magic, "KSEQ1\0\0\0", 8) != 0) throw std::runtime_error("not a .kseq file (bad magic)");
-        int32_t n_frames = 0, reserved = 0;
+        bool v2 = false;
         double l2b[7], start[7];
-        read_exact(f, &n_frames, 1, "the header"), read_exact(f, &reserved, 1, "the header");
-        read_exact(f, l2b, 7, "lidar_to_base"), read_exact(f, start, 7, "the start pose");
-        if (n_frames < 0 || n_frames > (1 << 24)) throw std::runtime_error("implausible frame count");
-        std::vector<Frame> frames((size_t)n_frames);
+        std::vector<Frame> frames;  // KSEQ1 / KSEQ2
+        kicp::Kseq3Drive drive;     // KSEQ3
         int64_t total_points = 0;
-        for (auto &fr : frames) {
-            if (v2) {
-                int32_t h[8];  // n, point_step, offset_x, offset_y, offset_z, stamp_datatype, stamp_offset, reserved
-                read_exact(f, h, 8, "a frame header");
-                read_exact(f, &fr.header_stamp, 1, "a frame header"), read_exact(f, fr.odom, 7, "a frame header");
-                if (h[0] < 0 || h[1] <= 0) throw std::runtime_error("bad point count or point_step");
-                fr.n = h[0];
-                const size_t bytes = (size_t)h[0] * (size_t)h[1];
-                uint8_t *raw = static_cast<uint8_t *>(host_alloc(bytes, pinned));
-                read_exact(f, raw, bytes, "records");
-                fr.msg.data = raw, fr.msg.width = (uint32_t)h[0], fr.msg.height = 1, fr.msg.point_step = (uint32_t)h[1];
-                fr.msg.fields = {{"x", (uint32_t)h[2], kicp::PF_FLOAT32, 1}, {"y", (uint32_t)h[3], kicp::PF_FLOAT32, 1},
-                                 {"z", (uint32_t)h[4], kicp::PF_FLOAT32, 1}};
-                if (h[5] != 0) fr.msg.fields.push_back({"t", (uint32_t)h[6], (uint8_t)h[5], 1});
-                total_points += fr.n;
-                continue;
-            }
-            read_exact(f, &fr.n, 1, "a frame header"), read_exact(f, &fr.has_stamps, 1, "a frame header");
-            read_exact(f, &fr.header_stamp, 1, "a frame header"), read_exact(f, fr.odom, 7, "a frame header");
-            if (fr.n < 0) throw std::runtime_error("negative point count");
-            fr.xyz = static_cast<float *>(host_alloc((size_t)fr.n * 3 * sizeof(float), pinned));
-            read_exact(f, fr.xyz, (size_t)fr.n * 3, "points");
-            if (fr.has_stamps) {
-                fr.stamps = static_cast<double *>(host_alloc((size_t)fr.n * sizeof(double), pinned));
-                read_exact(f, fr.stamps, (size_t)fr.n, "stamps");
-            }
-            total_points += fr.n;
+        if (v3) {
+            drive = kicp::read_kseq3(argv[1], [&](size_t bytes) { return host_alloc(bytes, pinned); });
+            std::memcpy(start, drive.start_pose, sizeof(start));
+            for (const auto &fr : drive.frames)
+                for (const auto &s : fr.sensors) total_points += staged_points(s);
+        } else {
+            v2 = read_kseq12(argv[1], pinned, l2b, start, frames, total_points);
         }
-        std::fclose(f);
-        if (publish != "none" && (!v2 || host_stamps)) throw std::runtime_error("--publish replays a KSEQ2 drive staged (without --host-stamps)");
-        if (device_input && !v2) throw std::runtime_error("--device-input replays a KSEQ2 drive");
-        // --device-input: every frame's records, as a GPU producer would leave them, on the default context's device (current since
-        // kicp::default_context() created it)
+        const int32_t n_frames = static_cast<int32_t>(v3 ? drive.frames.size() : frames.size());
+        if (publish != "none" && ((!v2 && !v3) || host_stamps))
+            throw std::runtime_error("--publish replays a KSEQ2 or KSEQ3 drive staged (without --host-stamps)");
+        if (device_input && !v2 && !v3) throw std::runtime_error("--device-input replays a KSEQ2 or KSEQ3 drive");
+        // --device-input: every frame's records (KSEQ3: every message's records or ranges), as a GPU producer would leave them, on the
+        // default context's device (current since kicp::default_context() created it)
         std::vector<void *> device_records;
-        for (auto &fr : frames) {
-            if (!device_input) break;
-            const size_t bytes = fr.msg.num_points() * fr.msg.point_step;
+        auto to_device = [&](const void *src, size_t bytes) {
             void *d = nullptr;
             cuda_check(cudaMalloc(&d, std::max<size_t>(bytes, 1)), "cudaMalloc");
             device_records.push_back(d);
-            cuda_check(cudaMemcpy(d, fr.msg.data, bytes, cudaMemcpyHostToDevice), "cudaMemcpy");
+            cuda_check(cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice), "cudaMemcpy");
+            return d;
+        };
+        for (auto &fr : frames) {
+            if (!device_input) break;
             fr.device_msg = fr.msg;
-            fr.device_msg.data = static_cast<const uint8_t *>(d);
+            fr.device_msg.data = static_cast<const uint8_t *>(to_device(fr.msg.data, fr.msg.num_points() * fr.msg.point_step));
         }
+        std::vector<std::vector<kicp::SensorFrame>> device_sensors;  // KSEQ3 --device-input: per frame, the messages in device memory
+        for (const auto &fr : drive.frames) {
+            if (!device_input) break;
+            device_sensors.push_back(fr.sensors);
+            for (auto &s : device_sensors.back()) {
+                s.device = true;
+                if (s.kind == kicp::SensorFrame::Kind::LaserScan)
+                    s.scan.ranges = static_cast<const float *>(to_device(s.scan.ranges, s.scan.n * sizeof(float)));
+                else
+                    s.cloud.data = static_cast<const uint8_t *>(to_device(s.cloud.data, s.cloud.num_points() * s.cloud.point_step));
+            }
+        }
+        // KSEQ3: the slots' extrinsics, every frame's odometry and samples, as the facade takes them
+        std::vector<Sophus::SE3d> lidar_to_bases;
+        for (const auto &slot : drive.slots) lidar_to_bases.push_back(kicp::from_pose7(slot.lidar_to_base));
+        std::vector<Sophus::SE3d> odoms;
+        std::vector<std::vector<kicp::OdometrySample>> samples(drive.frames.size());
+        int64_t total_samples = 0;
+        for (size_t k = 0; k < drive.frames.size(); ++k) {
+            odoms.push_back(kicp::from_pose7(drive.frames[k].relative_odometry));
+            for (const auto &s : drive.frames[k].samples) samples[k].push_back({s.stamp, kicp::from_pose7(s.pose)});
+            total_samples += static_cast<int64_t>(samples[k].size());
+        }
+        double first_header = 0.0;  // KSEQ3: where the first sweep begins, the earliest header stamp of the first frame
+        for (size_t s = 0; !drive.frames.empty() && s < drive.slots.size(); ++s)
+            first_header = s ? std::min(first_header, drive.frames[0].sensors[s].header_stamp) : drive.frames[0].sensors[0].header_stamp;
 
-        const Sophus::SE3d lidar_to_base = kicp::from_pose7(l2b);
+        const Sophus::SE3d lidar_to_base = v3 ? Sophus::SE3d() : kicp::from_pose7(l2b);
         std::vector<std::pair<double, Sophus::SE3d>> poses;
         double seconds = 0.0;
         std::vector<uint64_t> digests;
@@ -240,12 +336,73 @@ int main(int argc, char **argv) {
             kinematic_icp::pipeline::KinematicICP pipeline(config);
             pipeline.SetPose(kicp::from_pose7(start));
             poses.clear();
-            poses.reserve(frames.size());
+            poses.reserve((size_t)n_frames);
             digests.clear();
             live_written = live_records = 0;
             map_seconds = 0.0;
-            double last_processed = 0.0;  // end of the previous sweep (TimeStampHandler's state)
+            double last_processed = v3 ? first_header : 0.0;  // end of the previous sweep (TimeStampHandler's state)
+            // the staged frame's registration and, with --publish, the three clouds an online node publishes: reg() registers it as
+            // RegisterStagedFrame* does, reg_pc2() as RegisterStagedFramePointCloud2 does
+            auto register_staged = [&](auto &&reg, auto &&reg_pc2) {
+                if (publish == "none") {
+                    reg();
+                    return;
+                }
+                kicp::PointCloud2Data frame_msg, keypoints_msg, map_msg;
+                if (publish == "host") {
+                    const auto [frame, keypoints] = reg();
+                    frame_msg = eigen_to_pointcloud2(frame), keypoints_msg = eigen_to_pointcloud2(keypoints);
+                    const auto m0 = std::chrono::steady_clock::now();
+                    map_msg = eigen_to_pointcloud2(pipeline.LocalMap());
+                    map_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - m0).count();
+                } else if (publish == "device") {
+                    std::tie(frame_msg, keypoints_msg) = reg_pc2();
+                    const auto m0 = std::chrono::steady_clock::now();
+                    map_msg = pipeline.LocalMapPointCloud2();
+                    map_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - m0).count();
+                } else {
+                    std::tie(frame_msg, keypoints_msg) = reg_pc2();
+                    const auto m0 = std::chrono::steady_clock::now();
+                    const auto [view, stats] = pipeline.LocalMapPointCloud2Live();
+                    map_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - m0).count();
+                    live_written += stats.written, live_records += view.width;
+                    if (!digest_path.empty()) map_msg.data.assign(view.data, view.data + 12 * (size_t)view.width);  // hashing only
+                }
+                if (!digest_path.empty())
+                    digests.push_back(fnv1a(sorted_records(map_msg.data), fnv1a(keypoints_msg.data, fnv1a(frame_msg.data, 0xCBF29CE484222325ull))));
+            };
             const auto t0 = std::chrono::steady_clock::now();
+            for (size_t k = 0; v3 && k < drive.frames.size(); ++k) {
+                const std::vector<kicp::SensorFrame> &sensors = device_input ? device_sensors[k] : drive.frames[k].sensors;
+                const std::vector<kicp::OdometrySample> &smp = samples[k];
+                const Sophus::SE3d &odom = odoms[k];
+                try {
+                    if (sensors.size() == 1) {  // the single-sensor calls: bit for bit the KSEQ2 replay of the same records
+                        const kicp::SensorFrame &s = sensors[0];
+                        if (s.kind == kicp::SensorFrame::Kind::LaserScan)
+                            device_input ? pipeline.StageDeviceLaserScan(s.scan, s.header_stamp, last_processed)
+                                         : pipeline.StageLaserScan(s.scan, s.header_stamp, last_processed);
+                        else
+                            device_input ? pipeline.StageDeviceFrame(s.cloud, s.header_stamp, last_processed)
+                                         : pipeline.StageFrame(s.cloud, s.header_stamp, last_processed);
+                        register_staged(
+                            [&] { return smp.empty() ? pipeline.RegisterStagedFrame(lidar_to_bases[0], odom)
+                                                     : pipeline.RegisterStagedFrame(lidar_to_bases[0], odom, smp); },
+                            [&] { return smp.empty() ? pipeline.RegisterStagedFramePointCloud2(lidar_to_bases[0], odom)
+                                                     : pipeline.RegisterStagedFramePointCloud2(lidar_to_bases[0], odom, smp); });
+                    } else {
+                        pipeline.StageSensors(sensors, last_processed);
+                        register_staged(
+                            [&] { return smp.empty() ? pipeline.RegisterStagedSensors(lidar_to_bases, odom)
+                                                     : pipeline.RegisterStagedSensors(lidar_to_bases, odom, smp); },
+                            [&] { return smp.empty() ? pipeline.RegisterStagedSensorsPointCloud2(lidar_to_bases, odom)
+                                                     : pipeline.RegisterStagedSensorsPointCloud2(lidar_to_bases, odom, smp); });
+                    }
+                } catch (const std::exception &e) {
+                    throw std::runtime_error("frame " + std::to_string(k) + ": " + e.what());
+                }
+                poses.emplace_back(last_processed, pipeline.pose());  // the end of the sweep, as the offline node stamps its poses
+            }
             for (const auto &fr : frames) {
                 if (v2 && host_stamps) {
                     std::vector<double> stamps = kicp::extract_timestamps(fr.msg);
@@ -262,32 +419,8 @@ int main(int argc, char **argv) {
                     else
                         pipeline.StageFrame(fr.msg, fr.header_stamp, last_processed);  // the interval an online node looks the odometry up for
                     const Sophus::SE3d odom = kicp::from_pose7(fr.odom);
-                    if (publish == "none") {
-                        pipeline.RegisterStagedFrame(lidar_to_base, odom);
-                    } else {
-                        kicp::PointCloud2Data frame_msg, keypoints_msg, map_msg;
-                        if (publish == "host") {
-                            const auto [frame, keypoints] = pipeline.RegisterStagedFrame(lidar_to_base, odom);
-                            frame_msg = eigen_to_pointcloud2(frame), keypoints_msg = eigen_to_pointcloud2(keypoints);
-                            const auto m0 = std::chrono::steady_clock::now();
-                            map_msg = eigen_to_pointcloud2(pipeline.LocalMap());
-                            map_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - m0).count();
-                        } else if (publish == "device") {
-                            std::tie(frame_msg, keypoints_msg) = pipeline.RegisterStagedFramePointCloud2(lidar_to_base, odom);
-                            const auto m0 = std::chrono::steady_clock::now();
-                            map_msg = pipeline.LocalMapPointCloud2();
-                            map_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - m0).count();
-                        } else {
-                            std::tie(frame_msg, keypoints_msg) = pipeline.RegisterStagedFramePointCloud2(lidar_to_base, odom);
-                            const auto m0 = std::chrono::steady_clock::now();
-                            const auto [view, stats] = pipeline.LocalMapPointCloud2Live();
-                            map_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - m0).count();
-                            live_written += stats.written, live_records += view.width;
-                            if (!digest_path.empty()) map_msg.data.assign(view.data, view.data + 12 * (size_t)view.width);  // hashing only
-                        }
-                        if (!digest_path.empty())
-                            digests.push_back(fnv1a(sorted_records(map_msg.data), fnv1a(keypoints_msg.data, fnv1a(frame_msg.data, 0xCBF29CE484222325ull))));
-                    }
+                    register_staged([&] { return pipeline.RegisterStagedFrame(lidar_to_base, odom); },
+                                    [&] { return pipeline.RegisterStagedFramePointCloud2(lidar_to_base, odom); });
                     poses.emplace_back(fr.header_stamp, pipeline.pose());
                     continue;
                 }
@@ -331,12 +464,20 @@ int main(int argc, char **argv) {
                           n_frames ? (double)live_written / n_frames : 0.0, n_frames ? (double)live_records / n_frames : 0.0);
             live += buf;
         }
+        if (v3) {  // the slots, their kinds, and the odometry samples per frame (0: one motion per frame)
+            live += ", \"slots\": " + std::to_string(drive.slots.size()) + ", \"slot_kinds\": [";
+            for (size_t s = 0; s < drive.slots.size(); ++s)
+                live += std::string(s ? ", " : "") + (drive.slots[s].kind == kicp::KseqSlot::LaserScan ? "\"laser_scan\"" : "\"records\"");
+            char buf[64];
+            std::snprintf(buf, sizeof(buf), "], \"odometry_samples_per_frame\": %.2f", n_frames ? (double)total_samples / n_frames : 0.0);
+            live += buf;
+        }
         std::printf("{\"harness\": \"kicp_replay\", \"frames\": %d, \"points_per_frame\": %.0f, \"seconds\": %.6f, \"frames_per_s\": %.2f, "
                     "\"ms_per_frame\": %.4f, \"frames_per_s_best\": %.2f, \"repetition_seconds\": %s, \"host_buffers\": \"%s %s\", "
                     "\"deskew\": %s, \"publish\": \"%s\"%s, \"map_points\": %lld, \"tum_file\": \"%s\"}\n",
                     n_frames, n_frames ? (double)total_points / n_frames : 0.0, seconds, seconds > 0 ? n_frames / seconds : 0.0,
                     n_frames ? 1e3 * seconds / n_frames : 0.0, best > 0 ? n_frames / best : 0.0, reps.c_str(), pinned ? "pinned" : "pageable",
-                    !v2 ? "float32" : host_stamps ? "records, host-decoded stamps" : device_input ? "records, staged from device memory" : "records, staged",
+                    !v2 && !v3 ? "float32" : host_stamps ? "records, host-decoded stamps" : device_input ? "records, staged from device memory" : "records, staged",
                     config.deskew ? "true" : "false", publish.c_str(), live.c_str(), (long long)map_points, argv[2]);
         return 0;
     } catch (const std::exception &e) {
