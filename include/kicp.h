@@ -105,6 +105,14 @@ int kicp_stream_wait_ctx(kicp_ctx *ctx, void *stream);
  * library's own pipeline does.  Mode 1 restates that container from memory and is UNPINNED exactly as the test oracle's mode 1
  * is: pinning it means checking both against the library.  It accepts at most 2^28 points per down-sample (KICP_ERR_INVALID
  * beyond).  Other values fail with KICP_ERR_INVALID.
+ * "correspondences" 1 = every frame call (kicp_register_frame, kicp_register_staged_frame, _sensors and the _segments variants) also
+ * evaluates the registration source at the returned pose against the map BEFORE the frame's Update, by the rules of
+ * kicp_map_correspondences: two more kernel launches per frame, the pose read from the device result block and the source count from
+ * the device, and no further host synchronisation (the statistics come back with the frame's).  Read them with
+ * kicp_frame_correspondences / kicp_frame_correspondences_device.  The first frame (empty map) has no inliers and fitness 0; a frame
+ * that returns KICP_WARN_NO_CORRESPONDENCES is evaluated at its NaN pose, so every distance is DBL_MAX and a finite tau gives no
+ * inliers (the map stays untouched as always); with "frame_sync" 1 the count is the one read back mid-frame.  0 (default) = no launch,
+ * no allocation, nothing of any result changes.
  * Unknown names fail with KICP_ERR_INVALID.
  * Every setting but "downsample_order" computes the same result up to the summation order. */
 int kicp_ctx_set_option(kicp_ctx *ctx, const char *name, int32_t value);
@@ -208,6 +216,40 @@ int kicp_map_update_pose_device(kicp_map *map, const void *data, int64_t n, int3
  * unchanged until then (or kicp_ctx_synchronize): they are read in place. */
 int kicp_map_nearest_device_async(kicp_map *map, const void *data, int64_t n, int32_t dtype, int32_t point_step, int32_t offset_x,
                                   int32_t offset_y, int32_t offset_z, double *out_points, double *out_dist);
+
+/* ---- correspondences at a pose: how well a cloud fits the map at a pose, for instance how well a frame registered.
+ *      The reference's DataAssociation (registration/Registration.cpp:62-81) and the sums of ComputePerturbation (:86-118) evaluated
+ *      once at the pose T.  For source points p_i, i < n, a gate tau and the map:
+ *        q_i = T * p_i                          (the transform kicp_map_update_pose applies, bit for bit)
+ *        (n_i, d_i) = GetClosestNeighbor(q_i)   (kicp_map_nearest's rules and bits: (0,0,0), DBL_MAX for an empty neighbourhood)
+ *        inlier_i = d_i < tau                   (Registration.cpp:75; a NaN distance is not an inlier)
+ *      Over the inliers, with J = [R e_x | R (-p_y, p_x, 0)] and r = q_i - n_i (Registration.cpp:89-95):
+ *        sum_sq = sum |r|^2, jtj = {JTJ00, JTJ01, JTJ11}, jtr = {JTr0, JTr1}: ComputePerturbation's sums at T before the /N
+ *        normalisation, in the layout of the first five entries of kicp_reg_result.sums.
+ *      The sums are reduced in a fixed order (per-CTA partials, then one CTA adds them in index order, no floating-point atomics), so
+ *      repeated calls on the same inputs give the same bits.  The library derives no covariance from them (INTEGRATION.md shows one
+ *      way a node can). ------------------------------------------------------------------------------------------------------- */
+typedef struct kicp_corr_stats {
+    int64_t n_points;   /* n */
+    int64_t n_inliers;
+    double fitness;     /* n_inliers / n_points, 0 when n_points == 0 */
+    double inlier_rmse; /* sqrt(sum_sq / n_inliers), 0 without inliers */
+    double sum_sq;
+    double jtj[3];
+    double jtr[2];
+} kicp_corr_stats;
+/* n host points at xyz, pose double[7]; host outputs, each of which may be NULL: out_points n x 3 doubles (n_i), out_dist n doubles,
+ * out_inlier n bytes (1 = inlier), stats.  Mirrors kicp_map_nearest: one host synchronisation.  Errors: KICP_ERR_INVALID (kicp_last_error
+ * names the argument) for a null map or pose, n < 0, and xyz == NULL with n > 0. */
+int kicp_map_correspondences(kicp_map *map, const double *xyz, int64_t n, const double pose[7], double tau, double *out_points,
+                             double *out_dist, uint8_t *out_inlier, kicp_corr_stats *stats);
+/* The same for n device points in kicp_map_nearest_device_async's layout and validation rules, enqueued on the context stream with no
+ * host synchronisation.  Outputs may each be NULL: out_points / out_dist device memory of the context's device aligned to 8 bytes,
+ * out_inlier n bytes of such memory, stats device memory of the context's device or page-locked host memory (kicp_host_alloc),
+ * written on the context stream (valid after kicp_ctx_synchronize, or on a stream ordered by kicp_stream_wait_ctx). */
+int kicp_map_correspondences_device_async(kicp_map *map, const void *data, int64_t n, int32_t dtype, int32_t point_step, int32_t offset_x,
+                                          int32_t offset_y, int32_t offset_z, const double pose[7], double tau, double *out_points,
+                                          double *out_dist, uint8_t *out_inlier, kicp_corr_stats *stats);
 
 /* ---- kinematic_icp::KinematicRegistration::ComputeRobotMotion (registration/Registration.hpp:39-43,
  *      registration/Registration.cpp:151-190; single call site pipeline/KinematicICP.cpp:68-72) -------------- */
@@ -328,6 +370,15 @@ int kicp_frame_clouds_f32(kicp_ctx *ctx, const float **frame, int64_t *n_frame, 
  * Errors: KICP_ERR_INVALID for a null argument or another dtype. */
 int kicp_frame_clouds_device(kicp_ctx *ctx, int32_t dtype, const void **frame, int64_t *n_frame, const void **source,
                              int64_t *n_source);
+/* With option "correspondences" 1: the kicp_corr_stats of the last frame call on the context, its registration source evaluated at the
+ * returned pose against the map before that frame's Update.  All counts are 0 (and every field) when the option was off for that frame
+ * or the frame failed (any status but KICP_OK and KICP_WARN_NO_CORRESPONDENCES).  Errors: KICP_ERR_INVALID for a null argument,
+ * named by kicp_last_error. */
+int kicp_frame_correspondences(kicp_ctx *ctx, kicp_corr_stats *stats);
+/* The per-point results of that evaluation in context-owned device memory, one row per source point (kicp_frame_clouds_device's
+ * source, in its order): points n x 3 doubles, dist n doubles, inlier n bytes.  Lifetime and discard rules are kicp_frame_clouds_device's;
+ * *n is 0 when the option was off or the frame failed.  Errors: KICP_ERR_INVALID for a null argument, named by kicp_last_error. */
+int kicp_frame_correspondences_device(kicp_ctx *ctx, const double **points, const double **dist, const uint8_t **inlier, int64_t *n);
 
 /* ---- the same frame in two steps, for a caller that needs the sweep's time range before it has the relative odometry (the
  *      online server: ProcessTimestamps -> wheel-odometry lookup over [begin, end] -> RegisterFrame,

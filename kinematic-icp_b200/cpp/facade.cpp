@@ -25,6 +25,12 @@ kicp_ctx *default_context() {
             const std::string v = order;
             check(kicp_ctx_set_option(ctx, "downsample_order", v == "0" ? 0 : v == "1" ? 1 : -1), "KICP_DOWNSAMPLE_ORDER");
         }
+        // KICP_CORRESPONDENCES=0|1: context option "correspondences" (every frame reports its correspondences at the returned pose,
+        // KinematicICP::LastCorrespondenceStats); any other value throws
+        if (const char *corr = std::getenv("KICP_CORRESPONDENCES")) {
+            const std::string v = corr;
+            check(kicp_ctx_set_option(ctx, "correspondences", v == "0" ? 0 : v == "1" ? 1 : -1), "KICP_CORRESPONDENCES");
+        }
     });
     return ctx;
 }
@@ -230,6 +236,16 @@ std::tuple<kicp::PointCloud2Data, kicp::PointCloud2Data> KinematicICP::RegisterS
     const std::vector<Sophus::SE3d> &lidar_to_base, const Sophus::SE3d &relative_odometry, const std::vector<kicp::OdometrySample> &samples) {
     RegisterOnDevice(nullptr, lidar_to_base.data(), lidar_to_base.size(), true, relative_odometry, KICP_STAGE_F32, &samples);
     return StagedCloudsPointCloud2();
+}
+
+// the correspondence report of the last frame on the process-wide context (zero without option "correspondences")
+kicp_corr_stats KinematicICP::LastCorrespondenceStats() const {
+    kicp_corr_stats st{};
+    kicp::check(kicp_frame_correspondences(kicp::default_context(), &st), "kicp_frame_correspondences");
+    return st;
+}
+void KinematicICP::SetCorrespondences(bool on) {
+    kicp::check(kicp_ctx_set_option(kicp::default_context(), "correspondences", on ? 1 : 0), "kicp_ctx_set_option");
 }
 
 // the two clouds of the last frame, built in one pass each from the library's pinned staging

@@ -6,6 +6,9 @@
 // Both down-samples of RegisterFrame emit the order of first occurrence.  With KICP_DOWNSAMPLE_ORDER=1 in the environment when the
 // process-wide default context is created (kicp/runtime.hpp), they emit the iteration order of KISS-ICP v1.2.0's robin_map instead
 // (context option "downsample_order", include/kicp.h; unpinned like the test oracle's mode 1); a value other than 0 or 1 throws.
+// With KICP_CORRESPONDENCES=1 in the environment at that moment (or after KinematicICP::SetCorrespondences(true)), every frame also
+// reports its correspondences at the returned pose (context option "correspondences"), read with LastCorrespondenceStats; 0 leaves the
+// option off, any other value throws.
 #pragma once
 #include <Eigen/Core>
 #include <cmath>
@@ -132,6 +135,16 @@ public:
     // until the next call or the map's destruction.  A node keeps one PointCloud2 message and refills its data from the view before
     // each publication, or, with a zero-copy publisher, publishes the view's bytes directly.
     std::tuple<kicp::PointCloud2View, kicp_map_live_stats> LocalMapPointCloud2Live();
+
+    // Extension (not in the reference): how well the last frame registered.  With the report switched on, every RegisterFrame /
+    // RegisterStaged* call also evaluates its registration source at the returned pose against the local map as it was before the
+    // frame's update (context option "correspondences", include/kicp.h: two more kernel launches, no more host synchronisations).
+    // LastCorrespondenceStats returns kicp_frame_correspondences of the process-wide context: the last frame registered on it by any
+    // KinematicICP, all zero when the report was off or that frame failed.  Fitness, inlier RMSE, and J^T J / J^T r of
+    // ComputePerturbation at the returned pose, from which a node may build a covariance (INTEGRATION.md §10; the facade imposes
+    // none).  SetCorrespondences switches the report for the process-wide context, as KICP_CORRESPONDENCES does at its creation.
+    kicp_corr_stats LastCorrespondenceStats() const;
+    static void SetCorrespondences(bool on);
 
     void SetPose(const Sophus::SE3d &pose);  // also clears the map and the threshold statistics (KinematicICP.hpp:85-89)
 

@@ -6,6 +6,7 @@
 //
 //   kicp_replay drive.kseq out.tum [--deskew 0|1] [--voxel-size v] [--max-range r] [--min-range r] [--repeat k] [--pageable]
 //               [--host-stamps] [--device-input] [--publish host|device|live] [--publish-digest FILE] [--downsample-order 0|1]
+//               [--correspondences FILE]
 //
 // .kseq, little endian:  char magic[8] = "KSEQ1\0\0\0"; int32 n_frames; int32 reserved; double lidar_to_base[7]; double start_pose[7];
 //   per frame: int32 n_points; int32 has_stamps; double header_stamp; double relative_odometry[7]; float xyz[3 n]; double stamps[n] (if has_stamps)
@@ -32,6 +33,11 @@
 // may differ from run to run while its content does not.  The hashing is host work inside the timed loop: time without it.
 // --downsample-order 1 sets the default context's option "downsample_order" (kicp.h): both down-samples of every frame emit the
 // KISS-ICP robin_map order instead of the order of first occurrence (as KICP_DOWNSAMPLE_ORDER does for any facade program).
+// --correspondences FILE switches on the default context's option "correspondences" (kicp.h; KinematicICP::SetCorrespondences) and
+// writes one CSV line per frame of the last repetition, how well that frame registered (KinematicICP::LastCorrespondenceStats: its
+// registration source at the returned pose against the local map before the frame's update):
+//   stamp, n_points, n_inliers, fitness, inlier_rmse, JTJ00, JTJ01, JTJ11, JTr0, JTr1
+// the stamp as in the TUM file, the doubles with 17 significant digits (they read back to the same bits), no header line.
 //
 // Version 3, magic "KSEQ3\0\0\0", carries several message streams ("slots", 1..KICP_MAX_SENSORS: PointCloud2 records or 2D LaserScans,
 // each with its extrinsic) and the wheel odometry either as one relative motion or as poses sampled during the sweep:
@@ -206,14 +212,15 @@ int64_t staged_points(const kicp::SensorFrame &s) {
 int main(int argc, char **argv) {
     if (argc < 3) {
         std::fprintf(stderr, "usage: %s drive.kseq out.tum [--deskew 0|1] [--voxel-size v] [--max-range r] [--min-range r] [--repeat k] [--pageable] "
-                     "[--host-stamps] [--device-input] [--publish host|device|live] [--publish-digest FILE] [--downsample-order 0|1]\n", argv[0]);
+                     "[--host-stamps] [--device-input] [--publish host|device|live] [--publish-digest FILE] [--downsample-order 0|1] "
+                     "[--correspondences FILE]\n", argv[0]);
         return 2;
     }
     kinematic_icp::pipeline::Config config;  // the reference's defaults (pipeline/KinematicICP.hpp:38-60)
     config.deskew = true;
     int repeat = 1;
     bool pinned = true, host_stamps = false, device_input = false;
-    std::string publish = "none", digest_path;
+    std::string publish = "none", digest_path, corr_path;
     int downsample_order = -1;  // -1: leave the default context's option as it is
     for (int i = 3; i < argc; ++i) {
         const std::string a = argv[i];
@@ -232,6 +239,7 @@ int main(int argc, char **argv) {
             else if (a == "--device-input") device_input = true;
             else if (a == "--publish") publish = value("--publish");
             else if (a == "--publish-digest") digest_path = value("--publish-digest");
+            else if (a == "--correspondences") corr_path = value("--correspondences");
             else if (a == "--downsample-order") {
                 const std::string v = value("--downsample-order");
                 if (v != "0" && v != "1") throw std::runtime_error("--downsample-order takes 0 or 1");
@@ -265,6 +273,7 @@ int main(int argc, char **argv) {
         kicp::default_context();  // fails here, loudly, without a CUDA device
         if (downsample_order >= 0)
             kicp::check(kicp_ctx_set_option(kicp::default_context(), "downsample_order", downsample_order), "--downsample-order");
+        if (!corr_path.empty()) kinematic_icp::pipeline::KinematicICP::SetCorrespondences(true);
         bool v2 = false;
         double l2b[7], start[7];
         std::vector<Frame> frames;  // KSEQ1 / KSEQ2
@@ -328,6 +337,7 @@ int main(int argc, char **argv) {
         std::vector<std::pair<double, Sophus::SE3d>> poses;
         double seconds = 0.0;
         std::vector<uint64_t> digests;
+        std::vector<kicp_corr_stats> corr;  // --correspondences: every frame's report, in frame order (last repetition)
         int64_t map_points = 0;  // the local map's size after the last frame
         int64_t live_written = 0, live_records = 0;  // --publish live, last repetition: records written, and published, over all frames
         double map_seconds = 0.0;  // --publish, last repetition: time spent publishing the local map
@@ -338,6 +348,12 @@ int main(int argc, char **argv) {
             poses.clear();
             poses.reserve((size_t)n_frames);
             digests.clear();
+            corr.clear();
+            // after every frame: its pose with the stamp the TUM file carries, and with --correspondences its report
+            auto frame_done = [&](double stamp) {
+                poses.emplace_back(stamp, pipeline.pose());
+                if (!corr_path.empty()) corr.push_back(pipeline.LastCorrespondenceStats());
+            };
             live_written = live_records = 0;
             map_seconds = 0.0;
             double last_processed = v3 ? first_header : 0.0;  // end of the previous sweep (TimeStampHandler's state)
@@ -401,7 +417,7 @@ int main(int argc, char **argv) {
                 } catch (const std::exception &e) {
                     throw std::runtime_error("frame " + std::to_string(k) + ": " + e.what());
                 }
-                poses.emplace_back(last_processed, pipeline.pose());  // the end of the sweep, as the offline node stamps its poses
+                frame_done(last_processed);  // the end of the sweep, as the offline node stamps its poses
             }
             for (const auto &fr : frames) {
                 if (v2 && host_stamps) {
@@ -410,7 +426,7 @@ int main(int argc, char **argv) {
                     kicp_frame_input in = kicp::make_frame_input(fr.msg);
                     in.stamps = stamps.empty() ? nullptr : stamps.data(), in.n_stamps = (int64_t)stamps.size();
                     pipeline.RegisterFrame(in, lidar_to_base, kicp::from_pose7(fr.odom));
-                    poses.emplace_back(fr.header_stamp, pipeline.pose());
+                    frame_done(fr.header_stamp);
                     continue;
                 }
                 if (v2) {
@@ -421,14 +437,14 @@ int main(int argc, char **argv) {
                     const Sophus::SE3d odom = kicp::from_pose7(fr.odom);
                     register_staged([&] { return pipeline.RegisterStagedFrame(lidar_to_base, odom); },
                                     [&] { return pipeline.RegisterStagedFramePointCloud2(lidar_to_base, odom); });
-                    poses.emplace_back(fr.header_stamp, pipeline.pose());
+                    frame_done(fr.header_stamp);
                     continue;
                 }
                 kicp_frame_input in{};
                 in.data = fr.xyz, in.n = fr.n, in.dtype = KICP_DTYPE_F32, in.point_step = 0;
                 in.stamps = fr.has_stamps ? fr.stamps : nullptr, in.n_stamps = fr.has_stamps ? fr.n : 0;
                 pipeline.RegisterFrame(in, lidar_to_base, kicp::from_pose7(fr.odom));
-                poses.emplace_back(fr.header_stamp, pipeline.pose());
+                frame_done(fr.header_stamp);
             }
             seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
             rep_seconds.push_back(seconds);
@@ -451,6 +467,16 @@ int main(int argc, char **argv) {
             if (!d) throw std::runtime_error("cannot write " + digest_path);
             for (const uint64_t h : digests) std::fprintf(d, "%016llx\n", (unsigned long long)h);
             if (std::fclose(d) != 0) throw std::runtime_error("cannot write " + digest_path);
+        }
+        if (!corr_path.empty()) {
+            std::FILE *c = std::fopen(corr_path.c_str(), "w");
+            if (!c) throw std::runtime_error("cannot write " + corr_path);
+            for (size_t k = 0; k < corr.size(); ++k) {
+                const kicp_corr_stats &st = corr[k];
+                std::fprintf(c, "%.17g,%lld,%lld,%.17g,%.17g,%.17g,%.17g,%.17g,%.17g,%.17g\n", poses[k].first, (long long)st.n_points,
+                             (long long)st.n_inliers, st.fitness, st.inlier_rmse, st.jtj[0], st.jtj[1], st.jtj[2], st.jtr[0], st.jtr[1]);
+            }
+            if (std::fclose(c) != 0) throw std::runtime_error("cannot write " + corr_path);
         }
         std::string live;
         if (publish != "none") {

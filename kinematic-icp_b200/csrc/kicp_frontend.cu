@@ -150,6 +150,15 @@ struct Scratch {
     // other front-end call and after a frame that failed
     int64_t dev_n_frame = 0, dev_n_source = 0;
     bool dev_f32 = false;
+    // option "correspondences": the per-point results of the last frame's evaluation (allocated on first use for corr_cap points) and
+    // its statistics (pinned, copied on the stream); corr_n source points and `corr` as kicp_frame_correspondences returns them, 0 after
+    // any other front-end call, a frame that failed or one without the option
+    P3 *corr_pts = nullptr;
+    double *corr_dist = nullptr;
+    uint8_t *corr_inl = nullptr;
+    kicp_corr_stats *h_corr = nullptr;
+    int64_t corr_cap = 0, corr_n = 0;
+    kicp_corr_stats corr = {};
     double timing[8] = {0};  // host-side stage times of the last kicp_register_frame, milliseconds (debug export)
     int *first_idx = nullptr, *slot_of = nullptr, *d_count = nullptr;
     int4 *slots = nullptr;
@@ -171,6 +180,7 @@ void release(Scratch &s) {
     cudaFree(s.raw), cudaFreeHost(s.h_count), cudaFreeHost(s.h_mapctr), cudaFreeHost(s.h_range);
     cudaFree(s.d_seg_mm), cudaFree(s.d_seg_count), cudaFreeHost(s.h_seg_mm), cudaFreeHost(s.h_seg_count);
     cudaFree(s.d_segs), cudaFreeHost(s.h_segs);
+    cudaFree(s.corr_pts), cudaFree(s.corr_dist), cudaFree(s.corr_inl), cudaFreeHost(s.h_corr);
     if (s.ev_segs) cudaEventDestroy(s.ev_segs);
     s.staged.release();
     if (s.ev_front) cudaEventDestroy(s.ev_front);
@@ -284,6 +294,19 @@ int reserve_robin(kicp_ctx *c, Scratch &s) {
     KICP_CUDA(cudaMalloc(&s.ro_table, n * sizeof(int)));
     KICP_CUDA(cudaMemsetAsync(s.ro_cnt, 0, nb * sizeof(uint32_t), c->stream));
     s.ro_cap = s.cap;
+    return KICP_OK;
+}
+
+// the buffers of option "correspondences" for s.cap points (allocated on the first frame with the option, and after the scratch grew)
+int reserve_corr(Scratch &s) {
+    if (!s.h_corr) KICP_CUDA(cudaMallocHost(&s.h_corr, sizeof(kicp_corr_stats)));
+    if (s.corr_cap == s.cap) return KICP_OK;
+    cudaFree(s.corr_pts), cudaFree(s.corr_dist), cudaFree(s.corr_inl);
+    s.corr_pts = nullptr, s.corr_dist = nullptr, s.corr_inl = nullptr, s.corr_cap = 0;
+    KICP_CUDA(cudaMalloc(&s.corr_pts, (size_t)s.cap * sizeof(P3)));
+    KICP_CUDA(cudaMalloc(&s.corr_dist, (size_t)s.cap * sizeof(double)));
+    KICP_CUDA(cudaMalloc(&s.corr_inl, (size_t)s.cap));
+    s.corr_cap = s.cap;
     return KICP_OK;
 }
 
@@ -408,6 +431,7 @@ int open_frontend(kicp_ctx *c, int status, int64_t n) {
     if (c) {
         Scratch &s = scratch(c);
         s.held_n = -1, s.dev_n_frame = s.dev_n_source = 0;
+        s.corr_n = 0, s.corr = kicp_corr_stats{};
     }
     if (status != KICP_OK) return status;
     KICP_CUDA(cudaSetDevice(c->device));
@@ -620,6 +644,10 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
     const bool stage = (fp->stage_clouds & ~KICP_STAGE_F32) != 0 || a.out_frame || a.out_source;
     const bool stage32 = (fp->stage_clouds & KICP_STAGE_F32) != 0;
     const bool one_sync = n > 0 && !c->frame_sync && (!a.out_frame || a.cap_frame >= n) && (!a.out_source || a.cap_source >= n);
+    const bool corr = c->correspondences != 0;
+    s.corr_n = 0, s.corr = kicp_corr_stats{};
+    // the report's buffers are sized before anything of this frame is enqueued: a growth (cudaFree / cudaMalloc) waits for the device
+    if (corr) KICP_TRY(reserve_corr(s));
     // the survivor counts of the three stages (12 bytes back, one synchronisation of the stream)
     int counts[3] = {0, 0, 0};
     auto read_counts = [&]() -> int {
@@ -670,6 +698,14 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
     const int64_t src_copy = one_sync ? std::min<int64_t>(n, std::max<int64_t>(2 * s.last_source, 32768)) : counts[2];
     if (one_sync && (stage || stage32)) KICP_CUDA(cudaStreamWaitEvent(c->copy_stream, s.ev_front, 0));
     KICP_TRY(s.staged.fetch(c->copy_stream, s.out, s.out3, stage, stage32, one_sync ? n : counts[0], 0, src_copy));
+    if (corr) {
+        // the source at the pose the registration returns (read from its result block) against the map before this frame's Update,
+        // the source count read from the device in the single-synchronisation order; the statistics come back with the frame's
+        // synchronisation
+        KICP_TRY(kicp_map_enqueue_correspondences(map, reinterpret_cast<const double *>(s.out3), reg_n, one_sync ? s.d_count + 2 : nullptr,
+                                                  nullptr, kicp_device_result(c), a.tau, reinterpret_cast<double *>(s.corr_pts),
+                                                  s.corr_dist, s.corr_inl, s.h_corr));
+    }
     if (one_sync) {
         // local_map_.Update(frame_downsample, new_pose) (KinematicICP.cpp:79), pose and count still on the device
         KICP_TRY(kicp_map_update_pose_async(map, reinterpret_cast<const double *>(s.out2), n, s.d_count + 1, kicp_device_result(c),
@@ -694,7 +730,10 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
     if (counts[2] > src_copy) KICP_TRY(s.staged.fetch(c->copy_stream, s.out, s.out3, stage, stage32, 0, src_copy, counts[2]));
     if (stage || stage32 || !one_sync) KICP_CUDA(cudaStreamSynchronize(c->copy_stream));
     s.staged.publish(stage, stage32, counts[0], counts[2], a.out_frame, a.out_source);
-    if (status == KICP_OK || status == KICP_WARN_NO_CORRESPONDENCES) s.dev_n_frame = counts[0], s.dev_n_source = counts[2], s.dev_f32 = stage32;
+    if (status == KICP_OK || status == KICP_WARN_NO_CORRESPONDENCES) {
+        s.dev_n_frame = counts[0], s.dev_n_source = counts[2], s.dev_f32 = stage32;
+        if (corr) s.corr_n = counts[2], s.corr = *s.h_corr;
+    }
     s.timing[4] = ms_since();  // + clouds delivered
     return status;
 }
@@ -1214,6 +1253,29 @@ extern "C" int kicp_frame_clouds_device(kicp_ctx *c, int32_t dtype, const void *
     *frame = f64 ? static_cast<const void *>(s.out) : s.staged.d_rec;
     *source = f64 ? static_cast<const void *>(s.out3) : s.staged.d_rec ? s.staged.d_source_rec() : nullptr;
     *n_frame = ok ? s.dev_n_frame : 0, *n_source = ok ? s.dev_n_source : 0;
+    return KICP_OK;
+}
+
+// The correspondence report of the last frame (option "correspondences"): its statistics, and the per-point results in context-owned
+// device memory; not a front-end call
+extern "C" int kicp_frame_correspondences(kicp_ctx *c, kicp_corr_stats *stats) {
+    static const char fn[] = "kicp_frame_correspondences";
+    if (!stats) return kicp_invalid(fn, "stats: null pointer");
+    if (!c) return kicp_invalid(fn, "null context");
+    *stats = scratch(c).corr;
+    return KICP_OK;
+}
+extern "C" int kicp_frame_correspondences_device(kicp_ctx *c, const double **points, const double **dist, const uint8_t **inlier,
+                                                 int64_t *n) {
+    static const char fn[] = "kicp_frame_correspondences_device";
+    if (!points) return kicp_invalid(fn, "points: null pointer");
+    if (!dist) return kicp_invalid(fn, "dist: null pointer");
+    if (!inlier) return kicp_invalid(fn, "inlier: null pointer");
+    if (!n) return kicp_invalid(fn, "n: null pointer");
+    if (!c) return kicp_invalid(fn, "null context");
+    const Scratch &s = scratch(c);
+    *points = reinterpret_cast<const double *>(s.corr_pts), *dist = s.corr_dist, *inlier = s.corr_inl;
+    *n = s.corr_n;
     return KICP_OK;
 }
 

@@ -65,6 +65,7 @@ struct kicp_ctx {
     int nn_cache = 1;  // option "nn_cache"
     int frame_sync = 0;       // option "frame_sync": 1 = kicp_register_frame reads the survivor counts back mid-frame (legacy order)
     int downsample_order = 0;  // option "downsample_order": 1 = VoxelDownsample emits the robin_map's bucket order (kicp_frontend.cu)
+    int correspondences = 0;   // option "correspondences": 1 = the frame calls evaluate the source at the returned pose (kicp_frontend.cu)
     int overlap_upload = 1;
     // the registration's device state, neighbour cache, upload flags and profiling records (kicp_register_api.cu owns the type)
     struct RegScratch *reg = nullptr;
@@ -116,6 +117,13 @@ struct kicp_map {
     double *pts_spare = nullptr;
     // state of kicp_map_pointcloud_f32_live (kicp_map.cu), created by its first call
     struct MapLive *live = nullptr;
+    // correspondence report (kicp_map.cu, created by its first use): the per-CTA partials of k_corr_eval for corr_grid CTAs, the
+    // statistics k_corr_finish writes, and the inlier flags of host calls (corr_inl_cap bytes)
+    double *d_corr_part = nullptr;
+    kicp_corr_stats *d_corr_stats = nullptr;
+    uint8_t *d_corr_inl = nullptr;
+    int64_t corr_inl_cap = 0;
+    int corr_grid = 0;
     MapView view() const { return MapView{slots, nslots - 1, pts, (int)cap, voxel_size}; }
 };
 
@@ -189,6 +197,12 @@ const kicp_reg_result *kicp_device_result(kicp_ctx *c);
 // grid is planned for `n_hint` points, the count the producer expects, when that is smaller; 0 = no hint)
 int kicp_enqueue_registration_device(kicp_map *m, const double *d_xyz, int64_t n_max, const int *d_n, const double last[7],
                                      const double odom[7], double tau, const kicp_reg_params *p, int64_t n_hint);
+// defined in kicp_map.cu: the correspondence report of n_max device points (packed doubles) at `pose7` (host) or at the pose of the
+// result block `d_res`, the count min(*d_n, n_max) when d_n is given; per-point outputs may be null; the statistics are copied to
+// `stats` (device or page-locked host memory; may be null).  Two launches on the context stream, no host synchronisation.
+int kicp_map_enqueue_correspondences(kicp_map *m, const double *d_xyz, int64_t n_max, const int *d_n, const double *pose7,
+                                     const kicp_reg_result *d_res, double tau, double *d_points, double *d_dist, uint8_t *d_inlier,
+                                     kicp_corr_stats *stats);
 // creates / frees the registration's scratch (kicp_ctx::reg) with the context (kicp_register_api.cu)
 int kicp_reg_scratch_create(kicp_ctx *c);
 void kicp_reg_scratch_free(kicp_ctx *c);

@@ -416,6 +416,7 @@ extern "C" int kicp_map_destroy(kicp_map *m) {
     cudaStreamSynchronize(m->ctx->stream);
     cudaFree(m->slab), cudaFree(m->d_counters);
     cudaFree(m->d_in), cudaFree(m->d_xyz_t), cudaFree(m->d_next), cudaFree(m->d_touched), cudaFree(m->d_dist);
+    cudaFree(m->d_corr_part), cudaFree(m->d_corr_stats), cudaFree(m->d_corr_inl);
     map_live_free(m);
     delete m;
     return KICP_OK;
@@ -937,4 +938,106 @@ extern "C" int kicp_map_nearest_device_async(kicp_map *m, const void *data, int6
     KICP_TRY(map_device_points(m, in, packed, &q));
     KICP_CUDA(cudaSetDevice(m->ctx->device));
     return enqueue_nearest(m, q, n, out_points, out_dist);
+}
+
+// ---------------------------------------------------------------------------------------------------------- correspondences
+#include "kicp_corr_kernels.cuh"  // k_corr_eval, k_corr_finish
+
+// KICP_OK when `stats` is device memory of the context's device or page-locked host memory (what a copy on the stream can write
+// without waiting); otherwise KICP_ERR_INVALID naming it
+static int check_stats_memory(const kicp_ctx *c, const void *p, const char *what) {
+    cudaPointerAttributes at;
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+        cudaGetLastError();
+        return kicp_invalid(what, "not memory the CUDA runtime knows");
+    }
+    if (at.type == cudaMemoryTypeHost) return KICP_OK;
+    if (reinterpret_cast<uintptr_t>(p) % alignof(kicp_corr_stats)) return kicp_invalid(what, "not aligned to 8 bytes");
+    return kicp_check_device_range(c, p, sizeof(kicp_corr_stats), alignof(kicp_corr_stats), what);
+}
+
+// k_corr_eval's grid: as many 256-thread CTAs as are resident at once (the warps stride over the points beyond them), fewer for a
+// small n; the partials are allocated for the resident grid on first use
+static int corr_reserve(kicp_map *m) {
+    if (m->d_corr_part) return KICP_OK;
+    int per_sm = 0;
+    KICP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_corr_eval, kCorrThreads, 0));
+    const int grid = std::max(1, per_sm) * m->ctx->sm_count;
+    KICP_CUDA(cudaMalloc(&m->d_corr_part, (size_t)grid * kCorrStride * sizeof(double)));
+    KICP_CUDA(cudaMalloc(&m->d_corr_stats, sizeof(kicp_corr_stats)));
+    m->corr_grid = grid;
+    return KICP_OK;
+}
+
+int kicp_map_enqueue_correspondences(kicp_map *m, const double *d_xyz, int64_t n_max, const int *d_n, const double *pose7,
+                                     const kicp_reg_result *d_res, double tau, double *d_points, double *d_dist, uint8_t *d_inlier,
+                                     kicp_corr_stats *stats) {
+    kicp_ctx *c = m->ctx;
+    KICP_CUDA(cudaSetDevice(c->device));
+    KICP_TRY(corr_reserve(m));
+    const int per_cta = kCorrThreads / 32;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n_max + per_cta - 1) / per_cta, m->corr_grid));
+    Pose pose{0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0};
+    if (pose7) pose = Pose{pose7[0], pose7[1], pose7[2], pose7[3], pose7[4], pose7[5], pose7[6]};
+    k_corr_eval<<<grid, kCorrThreads, 0, c->stream>>>(m->view(), d_xyz, n_max, d_n, pose, d_res, tau, d_points, d_dist, d_inlier,
+                                                      m->d_corr_part);
+    KICP_CHECK_LAUNCH(c);
+    k_corr_finish<<<1, 32, 0, c->stream>>>(m->d_corr_part, grid, n_max, d_n, m->d_corr_stats);
+    KICP_CHECK_LAUNCH(c);
+    if (stats) KICP_CUDA(cudaMemcpyAsync(stats, m->d_corr_stats, sizeof(kicp_corr_stats), cudaMemcpyDefault, c->stream));
+    return KICP_OK;
+}
+
+// host points: copied into the map's input buffer, the per-point results into its own buffers (kicp_map_nearest's), then to the host
+extern "C" int kicp_map_correspondences(kicp_map *m, const double *xyz, int64_t n, const double pose[7], double tau, double *out_points,
+                                        double *out_dist, uint8_t *out_inlier, kicp_corr_stats *stats) {
+    static const char fn[] = "kicp_map_correspondences";
+    if (n < 0) return kicp_invalid(fn, "n < 0");
+    if (n > 0 && !xyz) return kicp_invalid(fn, "xyz: null pointer");
+    if (!pose) return kicp_invalid(fn, "pose: null pointer");
+    if (!m) return kicp_invalid(fn, "null map");
+    kicp_ctx *c = m->ctx;
+    KICP_CUDA(cudaSetDevice(c->device));
+    KICP_TRY(map_reserve_input(m, std::max<int64_t>(n, 1)));
+    if (out_inlier && n > m->corr_inl_cap) {
+        KICP_CUDA(cudaStreamSynchronize(c->stream));
+        cudaFree(m->d_corr_inl);
+        m->d_corr_inl = nullptr, m->corr_inl_cap = 0;
+        const int64_t cap = std::max<int64_t>(n + n / 4, 4096);
+        KICP_CUDA(cudaMalloc(&m->d_corr_inl, (size_t)cap));
+        m->corr_inl_cap = cap;
+    }
+    if (n) KICP_CUDA(cudaMemcpyAsync(m->d_in, xyz, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    KICP_TRY(kicp_map_enqueue_correspondences(m, m->d_in, n, nullptr, pose, nullptr, tau, out_points ? m->d_xyz_t : nullptr,
+                                              out_dist ? m->d_dist : nullptr, out_inlier ? m->d_corr_inl : nullptr, nullptr));
+    if (out_points && n) KICP_CUDA(cudaMemcpyAsync(out_points, m->d_xyz_t, (size_t)n * 3 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    if (out_dist && n) KICP_CUDA(cudaMemcpyAsync(out_dist, m->d_dist, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    if (out_inlier && n) KICP_CUDA(cudaMemcpyAsync(out_inlier, m->d_corr_inl, (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+    if (stats) KICP_CUDA(cudaMemcpyAsync(stats, m->d_corr_stats, sizeof(kicp_corr_stats), cudaMemcpyDeviceToHost, c->stream));
+    KICP_CUDA(cudaStreamSynchronize(c->stream));
+    return KICP_OK;
+}
+
+// device points: read in place (packed doubles) or widened into the map's input buffer; the results go straight to the caller's
+// memory, and nothing waits for them
+extern "C" int kicp_map_correspondences_device_async(kicp_map *m, const void *data, int64_t n, int32_t dtype, int32_t point_step,
+                                                     int32_t offset_x, int32_t offset_y, int32_t offset_z, const double pose[7], double tau,
+                                                     double *out_points, double *out_dist, uint8_t *out_inlier, kicp_corr_stats *stats) {
+    static const char fn[] = "kicp_map_correspondences_device_async";
+    const kicp_frame_input in{data, n, dtype, point_step, offset_x, offset_y, offset_z, nullptr, 0};
+    KICP_TRY(kicp_check_cloud_args(&in, fn));
+    if (!pose) return kicp_invalid(fn, "pose: null pointer");
+    if (!m) return kicp_invalid(fn, "null map");
+    bool packed = false;
+    KICP_TRY(kicp_check_device_cloud(m->ctx, &in, fn, &packed));
+    const std::string f(fn);
+    if (n > 0 && out_points)
+        KICP_TRY(kicp_check_device_range(m->ctx, out_points, (size_t)n * 3 * sizeof(double), sizeof(double), (f + ": out_points").c_str()));
+    if (n > 0 && out_dist)
+        KICP_TRY(kicp_check_device_range(m->ctx, out_dist, (size_t)n * sizeof(double), sizeof(double), (f + ": out_dist").c_str()));
+    if (n > 0 && out_inlier) KICP_TRY(kicp_check_device_range(m->ctx, out_inlier, (size_t)n, 1, (f + ": out_inlier").c_str()));
+    if (stats) KICP_TRY(check_stats_memory(m->ctx, stats, (f + ": stats").c_str()));
+    const double *q = nullptr;
+    KICP_TRY(map_device_points(m, in, packed, &q));
+    return kicp_map_enqueue_correspondences(m, q, n, nullptr, pose, nullptr, tau, out_points, out_dist, out_inlier, stats);
 }

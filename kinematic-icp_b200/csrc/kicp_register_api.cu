@@ -42,6 +42,9 @@ extern "C" int kicp_ctx_set_option(kicp_ctx *c, const char *name, int32_t value)
     } else if (!strcmp(name, "downsample_order")) {
         if (value != 0 && value != 1) return KICP_ERR_INVALID;
         c->downsample_order = value;
+    } else if (!strcmp(name, "correspondences")) {
+        if (value != 0 && value != 1) return KICP_ERR_INVALID;
+        c->correspondences = value;
     } else {
         kicp_set_error(std::string("kicp_ctx_set_option: unknown option ") + name);
         return KICP_ERR_INVALID;

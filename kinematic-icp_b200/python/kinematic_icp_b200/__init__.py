@@ -22,7 +22,25 @@ __all__ = ["Context", "VoxelHashMap", "Scan", "KinematicRegistration", "KicpErro
            "pinned_empty", "VoxelDownsample", "Preprocess",
            "RegisterFrame", "StageFrame", "StageLaserScan", "RegisterStagedFrame", "StagedFrame", "frame_clouds_f32",
            "frame_clouds_device", "PointCloudSensor", "LaserScanSensor", "StageSensors", "StagedSensors", "RegisterStagedSensors",
-           "RegisterStagedFrameSegments", "RegisterStagedSensorsSegments", "deskew_segments"]
+           "RegisterStagedFrameSegments", "RegisterStagedSensorsSegments", "deskew_segments", "CorrespondenceStats",
+           "frame_correspondences", "frame_correspondences_device"]
+
+
+class CorrespondenceStats(NamedTuple):
+    """kicp_corr_stats: a cloud's correspondences at a pose.  jtj = (JTJ00, JTJ01, JTJ11) and jtr = (JTr0, JTr1) are
+    ComputePerturbation's sums over the inliers before the /N normalisation (the layout of RegResult.sums[:, :5])."""
+    n_points: int
+    n_inliers: int
+    fitness: float
+    inlier_rmse: float
+    sum_sq: float
+    jtj: tuple
+    jtr: tuple
+
+    @classmethod
+    def from_c(cls, st):
+        return cls(int(st.n_points), int(st.n_inliers), float(st.fitness), float(st.inlier_rmse), float(st.sum_sq), tuple(st.jtj),
+                   tuple(st.jtr))
 
 
 class Context:
@@ -110,6 +128,9 @@ class Context:
                 self._device_scan.close()
                 self._device_scan = None
             lib().kicp_ctx_destroy(self.h)
+            if getattr(self, "_corr_stats", None) is not None:
+                self._corr_stats = None
+                lib().kicp_host_free(self._corr_stats_mem)
             self.h = C.c_void_p()
 
 
@@ -303,6 +324,73 @@ class VoxelHashMap:
         d = np.empty(len(q))
         check(lib().kicp_map_nearest(self.h, dp(q), len(q), dp(out), dp(d)), "kicp_map_nearest")
         return out, d
+
+
+    def Correspondences(self, points, pose, tau, *, out=None, stream=None, point_step=0, offsets=(0, 0, 0)):
+        """The correspondences of `points` at `pose` (kicp_map_correspondences): each point moved by the pose, its GetClosestNeighbor,
+        the gate distance < tau, and over the inliers the statistics of ComputePerturbation at that pose.  Returns (points (N, 3),
+        distances (N,), inlier (N,) uint8, CorrespondenceStats).
+
+        Device points (taken as AddPoints takes a device cloud) give device per-point results (kicp_map_correspondences_device_async):
+        the context waits for `stream`, then `stream` waits for the evaluation.  `out` = (points, distances, inlier), contiguous
+        float64 (N, 3), float64 (N,) and uint8 (N,) device arrays; without it torch tensors are allocated for torch points (any other
+        device array needs out).  The statistics are read back, so the call waits for the evaluation."""
+        pose = as_pose(pose)
+        tau = float(tau)
+        if _device.is_device(points):
+            d = _device.device_points(points, point_step, offsets)
+            what = "Correspondences"
+            if out is None:
+                out = (_device.empty_f64(points, (d.n, 3), what), _device.empty_f64(points, (d.n,), what), _device.empty_u8(points, d.n, what))
+            pts, dist, inl = out
+            pp = _device.output_f64(pts, (d.n, 3), what + ": out[0]")
+            pd = _device.output_f64(dist, (d.n,), what + ": out[1]")
+            pi = _device.output_u8(inl, d.n, what + ": out[2]")
+            s = _device.resolve_stream(stream, points)
+            self.ctx.wait_stream(s)
+            st = _pinned_corr_stats(self.ctx)
+            check(lib().kicp_map_correspondences_device_async(self.h, d.ptr, d.n, d.dtype, d.point_step, *d.offsets, dp(pose), tau, pp, pd,
+                                                              pi, C.addressof(st)), "kicp_map_correspondences_device_async")
+            self.ctx.stream_wait(s)
+            self.ctx.synchronize()
+            return pts, dist, inl, CorrespondenceStats.from_c(st)
+        _host_only("Correspondences", out=out, stream=stream, point_step=point_step)
+        q = as_points(points)
+        pts, dist, inl = np.empty_like(q), np.empty(len(q)), np.empty(len(q), np.uint8)
+        st = _capi.CorrStats()
+        check(lib().kicp_map_correspondences(self.h, dp(q), len(q), dp(pose), tau, dp(pts), dp(dist), inl.ctypes.data, C.byref(st)),
+              "kicp_map_correspondences")
+        return pts, dist, inl, CorrespondenceStats.from_c(st)
+
+
+def _pinned_corr_stats(ctx):
+    """a CorrStats in page-locked memory the context keeps (the stats of kicp_map_correspondences_device_async)"""
+    if getattr(ctx, "_corr_stats", None) is None:
+        p = C.c_void_p()
+        check(lib().kicp_host_alloc(C.sizeof(_capi.CorrStats), C.byref(p)), "kicp_host_alloc")
+        ctx._corr_stats_mem = p
+        ctx._corr_stats = _capi.CorrStats.from_address(p.value)
+    return ctx._corr_stats
+
+
+def frame_correspondences(ctx):
+    """CorrespondenceStats of the last frame registered on `ctx` with option "correspondences" 1 (kicp_frame_correspondences): its
+    registration source at the returned pose against the map before the frame's Update.  All zero when the option was off or the
+    frame failed."""
+    st = _capi.CorrStats()
+    check(lib().kicp_frame_correspondences(ctx.h, C.byref(st)), "kicp_frame_correspondences")
+    return CorrespondenceStats.from_c(st)
+
+
+def frame_correspondences_device(ctx):
+    """(points (n, 3) float64, distances (n,) float64, inlier (n,) uint8) of that evaluation, one row per source point, zero-copy in
+    context-owned device memory (kicp_frame_correspondences_device), with frame_clouds_device's lifetime: copy them to keep them."""
+    pp, pd, pi = C.c_void_p(), C.c_void_p(), C.c_void_p()
+    n = C.c_int64()
+    check(lib().kicp_frame_correspondences_device(ctx.h, C.byref(pp), C.byref(pd), C.byref(pi), C.byref(n)),
+          "kicp_frame_correspondences_device")
+    return (_device.DeviceArray(pp.value, (n.value, 3), "<f8", ctx), _device.DeviceArray(pd.value, (n.value,), "<f8", ctx),
+            _device.DeviceArray(pi.value, (n.value,), "|u1", ctx))
 
 
 class Scan:

@@ -50,6 +50,12 @@ class Profile(C.Structure):
                 ("assoc_iterations", C.c_int64)]
 
 
+class CorrStats(C.Structure):
+    """kicp_corr_stats: a cloud's correspondences at a pose (kicp_map_correspondences, option "correspondences" of the frame calls)"""
+    _fields_ = [("n_points", C.c_int64), ("n_inliers", C.c_int64), ("fitness", C.c_double), ("inlier_rmse", C.c_double),
+                ("sum_sq", C.c_double), ("jtj", C.c_double * 3), ("jtr", C.c_double * 2)]
+
+
 class FrameInput(C.Structure):
     """kicp_frame_input"""
     _fields_ = [("data", C.c_void_p), ("n", C.c_int64), ("dtype", C.c_int32), ("point_step", C.c_int32), ("offset_x", C.c_int32),
@@ -141,6 +147,9 @@ SYMBOLS = [
     ("kicp_map_update_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp]),
     ("kicp_map_update_pose_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp]),
     ("kicp_map_nearest_device_async", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    ("kicp_map_correspondences", C.c_int, [_P, c_dp, C.c_int64, c_dp, C.c_double, c_dp, c_dp, _P, C.POINTER(CorrStats)]),
+    ("kicp_map_correspondences_device_async", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp,
+                                                        C.c_double, _P, _P, _P, _P]),
     ("kicp_voxel_downsample_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, _P, C.c_int64, C.POINTER(C.c_int64)]),
     ("kicp_preprocess_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, c_dp, c_dp, C.c_double, C.c_double, C.c_int32, _P,
                                          C.c_int64, C.POINTER(C.c_int64)]),
@@ -165,6 +174,8 @@ SYMBOLS = [
     ("kicp_frame_clouds", C.c_int, [_P, C.POINTER(c_dp), C.POINTER(C.c_int64), C.POINTER(c_dp), C.POINTER(C.c_int64)]),
     ("kicp_frame_clouds_f32", C.c_int, [_P, C.POINTER(c_fp), C.POINTER(C.c_int64), C.POINTER(c_fp), C.POINTER(C.c_int64)]),
     ("kicp_frame_clouds_device", C.c_int, [_P, C.c_int32, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(_P), C.POINTER(C.c_int64)]),
+    ("kicp_frame_correspondences", C.c_int, [_P, C.POINTER(CorrStats)]),
+    ("kicp_frame_correspondences_device", C.c_int, [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_int64)]),
     ("kicp_frame_stage", C.c_int, [_P, C.POINTER(FrameInput), C.c_int32, C.c_int32, c_dp, C.POINTER(C.c_int64)]),
     ("kicp_frame_stage_device", C.c_int, [_P, C.POINTER(FrameInput), C.c_int32, C.c_int32, c_dp, C.POINTER(C.c_int64)]),
     ("kicp_register_staged_frame", C.c_int, [_P, c_dp, c_dp, c_dp, c_dp, C.c_double, C.POINTER(FrameParams), c_dp, c_dp, C.c_int64,

@@ -111,6 +111,22 @@ def output_f64(obj, shape, what):
     return int(cai["data"][0] or 0)
 
 
+def output_u8(obj, n, what):
+    """Pointer of `obj`, a contiguous uint8 device array of shape (n,)."""
+    cai = interface(obj)
+    if cai is None or cai["typestr"] != "|u1" or tuple(cai["shape"]) != (n,) or not _contiguous(cai):
+        raise ValueError("%s: expected a contiguous uint8 device array of shape (%d,)" % (what, n))
+    return int(cai["data"][0] or 0)
+
+
+def empty_u8(like, n, what):
+    """A new uint8 torch tensor of shape (n,) on the device of `like`, a torch tensor; any other device input needs out=."""
+    if not _is_torch_tensor(like):
+        raise ValueError("%s: pass out= for a device input that is not a torch tensor" % what)
+    import torch
+    return torch.empty((n,), dtype=torch.uint8, device=like.device)
+
+
 def empty_f64(like, shape, what):
     """A new float64 torch tensor of `shape` on the device of `like`, a torch tensor; any other device input needs out=."""
     if not _is_torch_tensor(like):
@@ -159,3 +175,19 @@ class DeviceCloud:
     def __cuda_array_interface__(self):
         return {"shape": self.shape, "typestr": "<f4" if self.dtype == KICP_DTYPE_F32 else "<f8",
                 "data": (self.ptr if self.n else 0, False), "version": 3, "strides": None, "stream": None}
+
+
+class DeviceArray:
+    """A zero-copy view of context-owned device memory of any shape and element type (`typestr`, e.g. "<f8", "|u1"), exposing
+    __cuda_array_interface__ like DeviceCloud, with DeviceCloud's lifetime rules."""
+
+    def __init__(self, ptr, shape, typestr, owner):
+        self.ptr, self.shape, self.typestr, self._owner = int(ptr or 0), tuple(int(s) for s in shape), typestr, owner
+
+    def __len__(self):
+        return self.shape[0]
+
+    @property
+    def __cuda_array_interface__(self):
+        return {"shape": self.shape, "typestr": self.typestr, "data": (self.ptr if self.shape[0] else 0, False), "version": 3,
+                "strides": None, "stream": None}
