@@ -251,6 +251,48 @@ int kicp_map_correspondences_device_async(kicp_map *map, const void *data, int64
                                           int32_t offset_y, int32_t offset_z, const double pose[7], double tau, double *out_points,
                                           double *out_dist, uint8_t *out_inlier, kicp_corr_stats *stats);
 
+/* ---- relocalisation: where a cloud fits the map around a prior pose (planar offsets x, y, yaw) ----------------------------------
+ * A hypothesis is an integer lattice point L = (ix, iy, ipsi) in units of u = step / 2^(levels-1) (the finest step).  Its pose is
+ * prior * Delta, Delta = (Rz(ipsi * u_yaw), (ix * u_x, iy * u_y, 0)), composed on the host as the C++ facade's Sophus product does
+ * (q = normalize(q_prior * (0, 0, sin(psi/2), cos(psi/2))), t = t_prior + q_prior * (x, y, 0)).  Its score is n_inliers (GetClosestNeighbor
+ * distance d < tau) and sum_sq (sum of d^2 over the inliers): the count and the distances are kicp_map_correspondences' at that pose
+ * bit for bit; sum_sq is added in an order of its own (fixed, so equal inputs give equal bits) and agrees with that report's sum to
+ * rounding.
+ * Ranking key: more inliers, smaller sum_sq, smaller |ipsi|, smaller ix^2 + iy^2, then (ipsi, ix, iy) lexicographic.
+ * Level 0 scores every lattice point of the box |x| <= half_extent[0] (likewise y, yaw) on the level-0 steps; level l >= 1 scores the
+ * 26 neighbours at the level's step (step / 2^l) of each of the `keep` best hypotheses so far, skipping points already scored. */
+typedef struct kicp_pose_search_params {
+    double half_extent[3]; /* x, y (m), yaw (rad) of level 0 around the prior; >= 0, yaw <= pi */
+    double step[3];        /* level-0 lattice steps, > 0 */
+    double tau;            /* inlier gate d < tau, > 0 */
+    int32_t levels;        /* 1..8 */
+    int32_t keep;          /* 1..64 */
+} kicp_pose_search_params;
+typedef struct kicp_pose_hypothesis {
+    double pose[7];     /* prior * Delta */
+    double offset[3];   /* x, y, yaw */
+    int32_t lattice[3]; /* ix, iy, ipsi in units of step / 2^(levels-1) */
+    int32_t level;      /* the level that scored it */
+    int64_t n_inliers;
+    double fitness;     /* n_inliers / n, 0 for n == 0 */
+    double inlier_rmse; /* sqrt(sum_sq / n_inliers), 0 without inliers */
+    double sum_sq;
+} kicp_pose_hypothesis;
+/* The best min(keep, n_scored) hypotheses by the key, over every distinct lattice point scored in the call, into out[0 .. *n_out)
+ * (cap >= keep entries); *n_scored (may be NULL) = the number of lattice points scored.  n host points in the robot base frame.
+ * Synchronous: one host synchronisation per level.  The map, a staged frame and the last frame's clouds and report are unchanged.
+ * n == 0 and an empty map are valid (every score (0, 0): the keep lattice points nearest the prior by the key).  KICP_ERR_INVALID,
+ * with kicp_last_error naming the argument, before any device work: a null map, prior, params, out or n_out; n < 0,
+ * n >= 2^40 (2^30 for device points) or xyz NULL with n > 0; a non-finite prior or parameter; a bound above; cap < keep; more than 4 194 304 level-0 hypotheses; lattice coordinates
+ * beyond int32. */
+int kicp_map_pose_search(kicp_map *map, const double *xyz, int64_t n, const double prior[7], const kicp_pose_search_params *params,
+                         kicp_pose_hypothesis *out, int32_t cap, int32_t *n_out, int64_t *n_scored);
+/* The same for n device points in kicp_map_nearest_device_async's layout and validation rules (packed float64 read in place, other
+ * layouts widened once into a buffer the map owns); the caller orders their producer before the call (kicp_ctx_wait_stream). */
+int kicp_map_pose_search_device(kicp_map *map, const void *data, int64_t n, int32_t dtype, int32_t point_step, int32_t offset_x,
+                                int32_t offset_y, int32_t offset_z, const double prior[7], const kicp_pose_search_params *params,
+                                kicp_pose_hypothesis *out, int32_t cap, int32_t *n_out, int64_t *n_scored);
+
 /* ---- kinematic_icp::KinematicRegistration::ComputeRobotMotion (registration/Registration.hpp:39-43,
  *      registration/Registration.cpp:151-190; single call site pipeline/KinematicICP.cpp:68-72) -------------- */
 /* frame: n host points in the robot base frame.  Returns last_robot_pose * relative_wheel_odometry when the map is

@@ -5,11 +5,25 @@
 #pragma once
 #include <Eigen/Core>
 #include <sophus/se3.hpp>
+#include <array>
 #include <tuple>
 #include <vector>
 
 #include "kicp/runtime.hpp"
 #include "kiss_icp/core/VoxelUtils.hpp"
+
+namespace kicp {
+// kicp_map_pose_search's parameters (x, y, yaw half extents and steps of level 0, the gate, levels, keep) and one returned hypothesis
+using PoseSearchParams = kicp_pose_search_params;
+struct PoseHypothesis {
+    Sophus::SE3d pose;                // prior * Delta
+    Eigen::Vector3d offset;           // x, y, yaw of Delta
+    std::array<int32_t, 3> lattice;   // ix, iy, ipsi in units of step / 2^(levels-1)
+    int level;
+    int64_t n_inliers;
+    double fitness, inlier_rmse, sum_sq;
+};
+}  // namespace kicp
 
 namespace kiss_icp {
 struct VoxelHashMap {
@@ -58,6 +72,28 @@ struct VoxelHashMap {
         double d = 0.0;
         kicp::check(kicp_map_nearest(handle_, query.data(), 1, p.data(), &d), "kicp_map_nearest");
         return std::make_tuple(p, d);
+    }
+
+    // Where `points` (robot base frame) fit the map around `prior`: the best hypotheses of kicp_map_pose_search, best first.  A node
+    // relocalises with `kicp.pose() = hyps[0].pose`, which keeps the map (SetPose clears it).
+    std::vector<kicp::PoseHypothesis> SearchPose(const std::vector<Eigen::Vector3d> &points, const Sophus::SE3d &prior,
+                                                 const kicp::PoseSearchParams &params) const {
+        double p[7];
+        kicp::to_pose7(prior, p);
+        std::vector<kicp_pose_hypothesis> h(params.keep > 0 ? (size_t)params.keep : 1);
+        int32_t n_out = 0;
+        int64_t n_scored = 0;
+        kicp::check(kicp_map_pose_search(handle_, kicp::xyz(points), (int64_t)points.size(), p, &params, h.data(), (int32_t)h.size(),
+                                         &n_out, &n_scored),
+                    "kicp_map_pose_search");
+        std::vector<kicp::PoseHypothesis> out;
+        for (int32_t i = 0; i < n_out; ++i) {
+            const kicp_pose_hypothesis &c = h[i];
+            out.push_back(kicp::PoseHypothesis{kicp::from_pose7(c.pose), Eigen::Vector3d(c.offset[0], c.offset[1], c.offset[2]),
+                                               {c.lattice[0], c.lattice[1], c.lattice[2]}, c.level, c.n_inliers, c.fitness,
+                                               c.inlier_rmse, c.sum_sq});
+        }
+        return out;
     }
 
     double voxel_size_;

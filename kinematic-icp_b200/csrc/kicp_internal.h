@@ -124,6 +124,8 @@ struct kicp_map {
     uint8_t *d_corr_inl = nullptr;
     int64_t corr_inl_cap = 0;
     int corr_grid = 0;
+    // scratch of kicp_map_pose_search* (kicp_map.cu, created by its first use, grown on demand)
+    struct PoseScratch *pose = nullptr;
     MapView view() const { return MapView{slots, nslots - 1, pts, (int)cap, voxel_size}; }
 };
 

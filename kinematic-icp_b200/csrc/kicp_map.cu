@@ -273,6 +273,7 @@ static int enqueue_exclusive_sum(kicp_ctx *c, const uint32_t *in, uint32_t *out,
 }
 
 static void map_live_free(kicp_map *m);  // state of kicp_map_pointcloud_f32_live, below
+static void pose_scratch_free(kicp_map *m);  // scratch of kicp_map_pose_search*, below
 
 // -------------------------------------------------------------------------------------------- host-side storage
 static uint32_t next_pow2(uint64_t v) {
@@ -418,6 +419,7 @@ extern "C" int kicp_map_destroy(kicp_map *m) {
     cudaFree(m->d_in), cudaFree(m->d_xyz_t), cudaFree(m->d_next), cudaFree(m->d_touched), cudaFree(m->d_dist);
     cudaFree(m->d_corr_part), cudaFree(m->d_corr_stats), cudaFree(m->d_corr_inl);
     map_live_free(m);
+    pose_scratch_free(m);
     delete m;
     return KICP_OK;
 }
@@ -1040,4 +1042,183 @@ extern "C" int kicp_map_correspondences_device_async(kicp_map *m, const void *da
     const double *q = nullptr;
     KICP_TRY(map_device_points(m, in, packed, &q));
     return kicp_map_enqueue_correspondences(m, q, n, nullptr, pose, nullptr, tau, out_points, out_dist, out_inlier, stats);
+}
+
+// ---------------------------------------------------------------------------------------------------------- pose search
+#include "kicp_pose_search_kernels.cuh"  // k_pose_score, k_pose_select; the host logic of kicp_pose_search.h
+
+// Device buffers of kicp_map_pose_search*, grown on demand and kept: the widened points, a level's tables, the scores and two entry
+// lists for k_pose_select's passes.  A repeated call of the same size allocates nothing.
+struct PoseScratch {
+    double *pts = nullptr, *rot = nullptr, *trans = nullptr, *sum = nullptr;
+    int32_t *pair_t = nullptr, *lat = nullptr, *tiles = nullptr;
+    int64_t *cnt = nullptr;
+    PsEntry *ent[2] = {nullptr, nullptr};
+    size_t pts_cap = 0, rot_cap = 0, trans_cap = 0, pair_cap = 0, lat_cap = 0, tiles_cap = 0, hyp_cap = 0, sum_cap = 0, ent_cap = 0;
+    int score_grid = 0;
+    PsTables tables;
+    std::vector<PsEntry> best;
+};
+
+static void pose_scratch_free(kicp_map *m) {
+    PoseScratch *S = m->pose;
+    if (!S) return;
+    cudaFree(S->pts), cudaFree(S->rot), cudaFree(S->trans), cudaFree(S->sum), cudaFree(S->pair_t), cudaFree(S->lat), cudaFree(S->tiles);
+    cudaFree(S->cnt), cudaFree(S->ent[0]), cudaFree(S->ent[1]);
+    delete S;
+    m->pose = nullptr;
+}
+
+// `p` holds at least `need` elements (growth by 1.25x; the stream is drained before a buffer it may use is freed)
+template <class T>
+static int ps_grow(kicp_ctx *c, T *&p, size_t &cap, size_t need) {
+    if (need <= cap) return KICP_OK;
+    KICP_CUDA(cudaStreamSynchronize(c->stream));
+    cudaFree(p);
+    p = nullptr, cap = 0;
+    const size_t n = std::max<size_t>(need + need / 4, 64);
+    KICP_CUDA(cudaMalloc(&p, n * sizeof(T)));
+    cap = n;
+    return KICP_OK;
+}
+
+template <class T>
+static int ps_upload(kicp_ctx *c, T *&d, size_t &cap, const std::vector<T> &h) {
+    KICP_TRY(ps_grow(c, d, cap, h.size()));
+    if (!h.empty()) KICP_CUDA(cudaMemcpyAsync(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, c->stream));
+    return KICP_OK;
+}
+
+// Scores `n_hyp` hypotheses of the tables on the device and returns the best `keep` of them (one synchronisation)
+static int ps_score_level(kicp_map *m, const double *d_pts, int64_t n, const PsPlan &P, bool level0, int64_t n_hyp,
+                          std::vector<PsEntry> &best) {
+    kicp_ctx *c = m->ctx;
+    PoseScratch &S = *m->pose;
+    KICP_TRY(ps_upload(c, S.rot, S.rot_cap, S.tables.rot));
+    KICP_TRY(ps_upload(c, S.trans, S.trans_cap, S.tables.trans));
+    int64_t n_tiles = 0;
+    if (level0) {
+        n_tiles = P.nr0 * ((P.nt0 + kPsTile - 1) / kPsTile);
+    } else {
+        KICP_TRY(ps_upload(c, S.pair_t, S.pair_cap, S.tables.pair_t));
+        KICP_TRY(ps_upload(c, S.lat, S.lat_cap, S.tables.lat));
+        KICP_TRY(ps_upload(c, S.tiles, S.tiles_cap, S.tables.tiles));
+        n_tiles = (int64_t)S.tables.tiles.size() / 3;
+    }
+    const int per_cta = kPsThreads * kPsSelectItems;
+    const int64_t parts = (n_hyp + per_cta - 1) / per_cta;
+    KICP_TRY(ps_grow(c, S.cnt, S.hyp_cap, (size_t)n_hyp));
+    KICP_TRY(ps_grow(c, S.sum, S.sum_cap, (size_t)n_hyp));
+    const size_t ent_need = (size_t)parts * P.keep;
+    if (ent_need > S.ent_cap) {
+        KICP_CUDA(cudaStreamSynchronize(c->stream));
+        cudaFree(S.ent[0]), cudaFree(S.ent[1]);
+        S.ent[0] = S.ent[1] = nullptr, S.ent_cap = 0;
+        const size_t e = ent_need + ent_need / 4;
+        KICP_CUDA(cudaMalloc(&S.ent[0], e * sizeof(PsEntry)));
+        KICP_CUDA(cudaMalloc(&S.ent[1], e * sizeof(PsEntry)));
+        S.ent_cap = e;
+    }
+    const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>(n_tiles, S.score_grid));
+    k_pose_score<<<grid, kPsThreads, 0, c->stream>>>(m->view(), d_pts, n, S.rot, S.trans, level0 ? (int32_t)P.nt0 : 0,
+                                                     level0 ? nullptr : S.pair_t, level0 ? nullptr : S.tiles, n_tiles, P.tau, S.cnt, S.sum);
+    KICP_CHECK_LAUNCH(c);
+    k_pose_select<<<(unsigned)parts, kPsThreads, 0, c->stream>>>(S.cnt, S.sum, level0 ? nullptr : S.lat, P.g, nullptr, n_hyp, per_cta,
+                                                                  P.keep, S.ent[0]);
+    KICP_CHECK_LAUNCH(c);
+    int cur = 0;
+    for (int64_t items = parts * P.keep; items > P.keep; items = ((items + per_cta - 1) / per_cta) * P.keep) {  // lists of lists
+        const unsigned g = (unsigned)((items + per_cta - 1) / per_cta);
+        k_pose_select<<<g, kPsThreads, 0, c->stream>>>(nullptr, nullptr, nullptr, P.g, S.ent[cur], items, per_cta, P.keep, S.ent[cur ^ 1]);
+        KICP_CHECK_LAUNCH(c);
+        cur ^= 1;
+    }
+    best.resize(P.keep);
+    KICP_CUDA(cudaMemcpyAsync(best.data(), S.ent[cur], P.keep * sizeof(PsEntry), cudaMemcpyDeviceToHost, c->stream));
+    KICP_CUDA(cudaStreamSynchronize(c->stream));
+    return KICP_OK;
+}
+
+// The level loop over device points d_pts (packed doubles); validated arguments
+static int ps_search(kicp_map *m, const double *d_pts, int64_t n, const double prior[7], const PsPlan &P, kicp_pose_hypothesis *out,
+                     int32_t *n_out, int64_t *n_scored) {
+    PoseScratch &S = *m->pose;
+    ps_tables0(P, prior, S.tables);
+    std::vector<PsKept> kept;
+    KICP_TRY(ps_score_level(m, d_pts, n, P, true, P.n0, S.best));
+    ps_merge(kept, S.best, 0, P.keep);
+    PsScored scored{&P, {}, P.n0};
+    for (int level = 1; level < P.levels; ++level) {
+        std::vector<PsEntry> parents;
+        for (const PsKept &k : kept) parents.push_back(k.e);
+        const std::vector<std::array<int32_t, 3>> kids = ps_children(P, level, parents, scored);
+        if (kids.empty()) continue;
+        ps_tables(P, prior, kids, S.tables);
+        KICP_TRY(ps_score_level(m, d_pts, n, P, false, (int64_t)kids.size(), S.best));
+        ps_merge(kept, S.best, level, P.keep);
+    }
+    for (size_t i = 0; i < kept.size(); ++i) ps_output(P, prior, kept[i], n, &out[i]);
+    *n_out = (int32_t)kept.size();
+    if (n_scored) *n_scored = scored.count;
+    return KICP_OK;
+}
+
+// the checks shared by both entry points, before any device work (the map last, so that every argument check is reachable without
+// one); creates the scratch
+static int ps_prepare(kicp_map *m, const char *fn, const double *prior, const kicp_pose_search_params *params, kicp_pose_hypothesis *out,
+                      int32_t cap, int32_t *n_out, PsPlan *P) {
+    if (!prior) return kicp_invalid(fn, "prior: null pointer");
+    if (!params) return kicp_invalid(fn, "params: null pointer");
+    if (!out) return kicp_invalid(fn, "out: null pointer");
+    if (!n_out) return kicp_invalid(fn, "n_out: null pointer");
+    for (int k = 0; k < 7; ++k)
+        if (!std::isfinite(prior[k])) return kicp_invalid(fn, "prior: not finite");
+    const std::string why = ps_plan(params, cap, P);
+    if (!why.empty()) return kicp_invalid(fn, why.c_str());
+    if (!m) return kicp_invalid(fn, "null map");
+    KICP_CUDA(cudaSetDevice(m->ctx->device));
+    if (!m->pose) {  // the scratch is attached only once its grid is known, so a failed occupancy query is reported every call
+        int per_sm = 0;
+        KICP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pose_score, kPsThreads, 0));
+        if (per_sm < 1) return kicp_invalid(fn, "k_pose_score cannot be resident on this device");
+        m->pose = new PoseScratch();
+        m->pose->score_grid = per_sm * m->ctx->sm_count;
+    }
+    return KICP_OK;
+}
+
+extern "C" int kicp_map_pose_search(kicp_map *m, const double *xyz, int64_t n, const double prior[7], const kicp_pose_search_params *params,
+                                    kicp_pose_hypothesis *out, int32_t cap, int32_t *n_out, int64_t *n_scored) {
+    static const char fn[] = "kicp_map_pose_search";
+    if (n < 0) return kicp_invalid(fn, "n < 0");
+    if (n >= kPsMaxPoints) return kicp_invalid(fn, "n: 2^40 points or more");
+    if (n > 0 && !xyz) return kicp_invalid(fn, "xyz: null pointer");
+    PsPlan P;
+    KICP_TRY(ps_prepare(m, fn, prior, params, out, cap, n_out, &P));
+    kicp_ctx *c = m->ctx;
+    PoseScratch &S = *m->pose;
+    KICP_TRY(ps_grow(c, S.pts, S.pts_cap, (size_t)std::max<int64_t>(n, 1) * 3));
+    if (n) KICP_CUDA(cudaMemcpyAsync(S.pts, xyz, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    return ps_search(m, S.pts, n, prior, P, out, n_out, n_scored);
+}
+
+extern "C" int kicp_map_pose_search_device(kicp_map *m, const void *data, int64_t n, int32_t dtype, int32_t point_step, int32_t offset_x,
+                                           int32_t offset_y, int32_t offset_z, const double prior[7], const kicp_pose_search_params *params,
+                                           kicp_pose_hypothesis *out, int32_t cap, int32_t *n_out, int64_t *n_scored) {
+    static const char fn[] = "kicp_map_pose_search_device";
+    const kicp_frame_input in{data, n, dtype, point_step, offset_x, offset_y, offset_z, nullptr, 0};
+    KICP_TRY(kicp_check_cloud_args(&in, fn));  // also n < 2^30, well inside kPsMaxPoints
+    PsPlan P;
+    KICP_TRY(ps_prepare(m, fn, prior, params, out, cap, n_out, &P));
+    bool packed = false;
+    KICP_TRY(kicp_check_device_cloud(m->ctx, &in, fn, &packed));
+    kicp_ctx *c = m->ctx;
+    PoseScratch &S = *m->pose;
+    const double *q = static_cast<const double *>(data);
+    if (!packed && n > 0) {  // widened once into the search's own buffer (the map's input buffer is left alone)
+        KICP_TRY(ps_grow(c, S.pts, S.pts_cap, (size_t)n * 3));
+        KICP_TRY(kicp_enqueue_widen(c, &in, S.pts));
+        q = S.pts;
+    }
+    return ps_search(m, q, n, prior, P, out, n_out, n_scored);
 }

@@ -23,7 +23,7 @@ __all__ = ["Context", "VoxelHashMap", "Scan", "KinematicRegistration", "KicpErro
            "RegisterFrame", "StageFrame", "StageLaserScan", "RegisterStagedFrame", "StagedFrame", "frame_clouds_f32",
            "frame_clouds_device", "PointCloudSensor", "LaserScanSensor", "StageSensors", "StagedSensors", "RegisterStagedSensors",
            "RegisterStagedFrameSegments", "RegisterStagedSensorsSegments", "deskew_segments", "CorrespondenceStats",
-           "frame_correspondences", "frame_correspondences_device"]
+           "frame_correspondences", "frame_correspondences_device", "PoseHypothesis"]
 
 
 class CorrespondenceStats(NamedTuple):
@@ -41,6 +41,24 @@ class CorrespondenceStats(NamedTuple):
     def from_c(cls, st):
         return cls(int(st.n_points), int(st.n_inliers), float(st.fitness), float(st.inlier_rmse), float(st.sum_sq), tuple(st.jtj),
                    tuple(st.jtr))
+
+
+class PoseHypothesis(NamedTuple):
+    """kicp_pose_hypothesis: a pose the pose search scored.  pose = prior * Delta (pose7), offset = (x, y, yaw) of Delta, lattice =
+    (ix, iy, ipsi) in units of step / 2^(levels-1), level = the level that scored it."""
+    pose: np.ndarray
+    offset: tuple
+    lattice: tuple
+    level: int
+    n_inliers: int
+    fitness: float
+    inlier_rmse: float
+    sum_sq: float
+
+    @classmethod
+    def from_c(cls, h):
+        return cls(np.array(h.pose[:]), tuple(h.offset), tuple(h.lattice), int(h.level), int(h.n_inliers), float(h.fitness),
+                   float(h.inlier_rmse), float(h.sum_sq))
 
 
 class Context:
@@ -361,6 +379,32 @@ class VoxelHashMap:
         check(lib().kicp_map_correspondences(self.h, dp(q), len(q), dp(pose), tau, dp(pts), dp(dist), inl.ctypes.data, C.byref(st)),
               "kicp_map_correspondences")
         return pts, dist, inl, CorrespondenceStats.from_c(st)
+
+    def PoseSearch(self, points, prior, tau, half_extent, step, levels=3, keep=8, *, stream=None, point_step=0, offsets=(0, 0, 0)):
+        """Where `points` (robot base frame) fit the map around `prior` (kicp_map_pose_search): a lattice of planar offsets (x, y,
+        yaw) of +-half_extent on `step` scored at level 0, then the 26 neighbours of the `keep` best at each finer level (step / 2^l).
+        A hypothesis's score is Correspondences(points, pose, tau)'s inlier count (exactly) and its sum of squared distances (to
+        rounding: it is added in an order of its own).  Returns (the best
+        min(keep, n_scored) as PoseHypothesis, best first; n_scored).  The map is not modified.
+
+        Device points (taken as AddPoints takes a device cloud) are read on the device (kicp_map_pose_search_device) after the
+        context has waited for `stream`."""
+        prior = as_pose(prior)
+        p = _capi.PoseSearchParams((C.c_double * 3)(*[float(v) for v in half_extent]), (C.c_double * 3)(*[float(v) for v in step]),
+                                   float(tau), int(levels), int(keep))
+        cap = max(int(keep), 1)
+        out = (_capi.PoseHypothesis * cap)()
+        n_out, n_scored = C.c_int32(), C.c_int64()
+        if _device.is_device(points):
+            d = self._device_points(points, stream, point_step, offsets)
+            check(lib().kicp_map_pose_search_device(self.h, d.ptr, d.n, d.dtype, d.point_step, *d.offsets, dp(prior), C.byref(p), out,
+                                                    cap, C.byref(n_out), C.byref(n_scored)), "kicp_map_pose_search_device")
+        else:
+            _host_only("PoseSearch", stream=stream, point_step=point_step)
+            q = as_points(points) if len(points) else np.zeros((0, 3))
+            check(lib().kicp_map_pose_search(self.h, dp(q), len(q), dp(prior), C.byref(p), out, cap, C.byref(n_out),
+                                             C.byref(n_scored)), "kicp_map_pose_search")
+        return [PoseHypothesis.from_c(out[i]) for i in range(n_out.value)], n_scored.value
 
 
 def _pinned_corr_stats(ctx):

@@ -56,6 +56,17 @@ class CorrStats(C.Structure):
                 ("sum_sq", C.c_double), ("jtj", C.c_double * 3), ("jtr", C.c_double * 2)]
 
 
+class PoseSearchParams(C.Structure):
+    """kicp_pose_search_params"""
+    _fields_ = [("half_extent", C.c_double * 3), ("step", C.c_double * 3), ("tau", C.c_double), ("levels", C.c_int32), ("keep", C.c_int32)]
+
+
+class PoseHypothesis(C.Structure):
+    """kicp_pose_hypothesis"""
+    _fields_ = [("pose", C.c_double * 7), ("offset", C.c_double * 3), ("lattice", C.c_int32 * 3), ("level", C.c_int32),
+                ("n_inliers", C.c_int64), ("fitness", C.c_double), ("inlier_rmse", C.c_double), ("sum_sq", C.c_double)]
+
+
 class FrameInput(C.Structure):
     """kicp_frame_input"""
     _fields_ = [("data", C.c_void_p), ("n", C.c_int64), ("dtype", C.c_int32), ("point_step", C.c_int32), ("offset_x", C.c_int32),
@@ -150,6 +161,11 @@ SYMBOLS = [
     ("kicp_map_correspondences", C.c_int, [_P, c_dp, C.c_int64, c_dp, C.c_double, c_dp, c_dp, _P, C.POINTER(CorrStats)]),
     ("kicp_map_correspondences_device_async", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp,
                                                         C.c_double, _P, _P, _P, _P]),
+    ("kicp_map_pose_search", C.c_int, [_P, c_dp, C.c_int64, c_dp, C.POINTER(PoseSearchParams), C.POINTER(PoseHypothesis), C.c_int32,
+                                       C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
+    ("kicp_map_pose_search_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp,
+                                              C.POINTER(PoseSearchParams), C.POINTER(PoseHypothesis), C.c_int32, C.POINTER(C.c_int32),
+                                              C.POINTER(C.c_int64)]),
     ("kicp_voxel_downsample_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, _P, C.c_int64, C.POINTER(C.c_int64)]),
     ("kicp_preprocess_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, c_dp, c_dp, C.c_double, C.c_double, C.c_int32, _P,
                                          C.c_int64, C.POINTER(C.c_int64)]),
