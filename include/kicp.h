@@ -293,6 +293,48 @@ int kicp_map_pose_search_device(kicp_map *map, const void *data, int64_t n, int3
                                 int32_t offset_y, int32_t offset_z, const double prior[7], const kicp_pose_search_params *params,
                                 kicp_pose_hypothesis *out, int32_t cap, int32_t *n_out, int64_t *n_scored);
 
+/* ---- planar alignment: Gauss-Newton in (x, y, yaw) of a cloud against the map from up to 64 starting poses -------------------
+ * Each starting pose T0 is aligned on its own: T = T0; for at most max_iterations steps, the inliers at T (q = T p, (nb, d) =
+ * GetClosestNeighbor(q), d < tau, r = q - nb, J = [R e_x | R e_y | R (-p_y, p_x, 0)]) give A = J^T J / N and b = J^T r / N, dx =
+ * -A^-1 b by a fixed LDL^T, and T = T * Delta with Delta = (R_q, (dx0, dx1, 0)), q = normalize((0, 0, dx2/2, 1)) (a turn by
+ * 2 atan(dx2/2): no trigonometry, the same fixed point).  It stops with CONVERGED when |dx| < convergence (after that step),
+ * NO_CORRESPONDENCES when no point is an inlier (n == 0 and an empty map included), SINGULAR when a pivot of the factorisation is not
+ * positive and finite or dx is not finite (both with T unchanged), else MAX_ITERATIONS.  The report is taken at the returned pose:
+ * n_inliers and the per-point distances are kicp_map_correspondences' at that pose exactly; the sums are added in an order that
+ * depends on n only, so an alignment's bits do not depend on the other starting poses of the call. */
+#define KICP_ALIGN_CONVERGED 0
+#define KICP_ALIGN_MAX_ITERATIONS 1
+#define KICP_ALIGN_NO_CORRESPONDENCES 2
+#define KICP_ALIGN_SINGULAR 3
+typedef struct kicp_planar_align_params {
+    double tau;             /* inlier gate d < tau: finite, > 0 */
+    double convergence;     /* stop when |dx| < convergence: finite, >= 0 (the reference's convergence_criterion: 1e-3) */
+    int32_t max_iterations; /* 1..KICP_MAX_ITERATIONS (the reference's max_num_iterations: 10) */
+} kicp_planar_align_params;
+typedef struct kicp_planar_alignment {
+    double pose[7];     /* the returned pose T */
+    int32_t status;     /* KICP_ALIGN_* */
+    int32_t iterations; /* updates applied */
+    double last_step;   /* |dx| of the last update, 0 without one */
+    int64_t n_inliers;  /* at pose */
+    double fitness;     /* n_inliers / n, 0 for n == 0 */
+    double inlier_rmse; /* sqrt(sum_sq / n_inliers), 0 without inliers */
+    double sum_sq;      /* sum of |r|^2 over the inliers */
+    double jtj[6];      /* J^T J over (x, y, yaw), unnormalised: {00, 01, 02, 11, 12, 22} */
+    double jtr[3];      /* J^T r, unnormalised */
+} kicp_planar_alignment;
+/* n host points in the robot base frame (n < 2^40), n_initial (1..64) starting poses initial[7 * k .. 7 * k + 6] -> out[k].
+ * Synchronous: one host synchronisation.  The map, a staged frame and the last frame's clouds and report are unchanged.
+ * KICP_ERR_INVALID, with kicp_last_error naming the argument, before any device work: a null map, initial, params or out; xyz NULL
+ * with n > 0; n < 0 or n >= 2^40; n_initial outside 1..64; a non-finite starting pose; a parameter outside its range above. */
+int kicp_map_align_planar(kicp_map *map, const double *xyz, int64_t n, const double *initial, int32_t n_initial,
+                          const kicp_planar_align_params *params, kicp_planar_alignment *out);
+/* The same for n device points in kicp_map_nearest_device_async's layout and validation rules (packed float64 read in place, other
+ * layouts widened once into a buffer the map owns); the caller orders their producer before the call (kicp_ctx_wait_stream). */
+int kicp_map_align_planar_device(kicp_map *map, const void *data, int64_t n, int32_t dtype, int32_t point_step, int32_t offset_x,
+                                 int32_t offset_y, int32_t offset_z, const double *initial, int32_t n_initial,
+                                 const kicp_planar_align_params *params, kicp_planar_alignment *out);
+
 /* ---- kinematic_icp::KinematicRegistration::ComputeRobotMotion (registration/Registration.hpp:39-43,
  *      registration/Registration.cpp:151-190; single call site pipeline/KinematicICP.cpp:68-72) -------------- */
 /* frame: n host points in the robot base frame.  Returns last_robot_pose * relative_wheel_odometry when the map is

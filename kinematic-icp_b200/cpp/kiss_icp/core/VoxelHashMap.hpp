@@ -5,6 +5,7 @@
 #pragma once
 #include <Eigen/Core>
 #include <sophus/se3.hpp>
+#include <algorithm>
 #include <array>
 #include <tuple>
 #include <vector>
@@ -22,6 +23,18 @@ struct PoseHypothesis {
     int level;
     int64_t n_inliers;
     double fitness, inlier_rmse, sum_sq;
+};
+// kicp_map_align_planar's parameters (gate, convergence, max_iterations) and one start's result
+using PlanarAlignParams = kicp_planar_align_params;
+struct PlanarAlignment {
+    Sophus::SE3d pose;  // the returned pose
+    int status;         // KICP_ALIGN_*
+    int iterations;
+    double last_step;
+    int64_t n_inliers;  // the correspondence report at `pose`
+    double fitness, inlier_rmse, sum_sq;
+    std::array<double, 6> jtj;  // J^T J over (x, y, yaw): 00, 01, 02, 11, 12, 22
+    std::array<double, 3> jtr;
 };
 }  // namespace kicp
 
@@ -92,6 +105,29 @@ struct VoxelHashMap {
             out.push_back(kicp::PoseHypothesis{kicp::from_pose7(c.pose), Eigen::Vector3d(c.offset[0], c.offset[1], c.offset[2]),
                                                {c.lattice[0], c.lattice[1], c.lattice[2]}, c.level, c.n_inliers, c.fitness,
                                                c.inlier_rmse, c.sum_sq});
+        }
+        return out;
+    }
+
+    // Gauss-Newton in (x, y, yaw) of `points` (robot base frame) against the map from each of `initial` (1 to 64 starts, each aligned
+    // on its own; kicp_map_align_planar), one result per start in input order.  After SearchPose: align its hypotheses' poses and
+    // pick the best result by the caller's rule.
+    std::vector<kicp::PlanarAlignment> AlignPlanar(const std::vector<Eigen::Vector3d> &points, const std::vector<Sophus::SE3d> &initial,
+                                                   const kicp::PlanarAlignParams &params) const {
+        std::vector<double> starts(7 * initial.size());
+        for (size_t k = 0; k < initial.size(); ++k) kicp::to_pose7(initial[k], &starts[7 * k]);
+        std::vector<kicp_planar_alignment> r(std::max<size_t>(initial.size(), 1));
+        kicp::check(kicp_map_align_planar(handle_, kicp::xyz(points), (int64_t)points.size(), starts.data(), (int32_t)initial.size(),
+                                          &params, r.data()),
+                    "kicp_map_align_planar");
+        std::vector<kicp::PlanarAlignment> out;
+        for (size_t k = 0; k < initial.size(); ++k) {
+            const kicp_planar_alignment &c = r[k];
+            kicp::PlanarAlignment a{kicp::from_pose7(c.pose), c.status, c.iterations, c.last_step, c.n_inliers, c.fitness,
+                                    c.inlier_rmse, c.sum_sq, {}, {}};
+            for (int j = 0; j < 6; ++j) a.jtj[j] = c.jtj[j];
+            for (int j = 0; j < 3; ++j) a.jtr[j] = c.jtr[j];
+            out.push_back(a);
         }
         return out;
     }

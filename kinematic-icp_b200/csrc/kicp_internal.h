@@ -126,6 +126,8 @@ struct kicp_map {
     int corr_grid = 0;
     // scratch of kicp_map_pose_search* (kicp_map.cu, created by its first use, grown on demand)
     struct PoseScratch *pose = nullptr;
+    // scratch of kicp_map_align_planar* (kicp_align.cu, created by its first use, grown on demand)
+    struct AlignScratch *align = nullptr;
     MapView view() const { return MapView{slots, nslots - 1, pts, (int)cap, voxel_size}; }
 };
 
@@ -177,6 +179,8 @@ int kicp_scan_reserve_bytes(kicp_scan *scan, int64_t bytes);
 int kicp_scan_set_layout(kicp_scan *scan, int32_t dtype, int32_t point_step, int32_t ox, int32_t oy, int32_t oz);
 // VoxelHashMap::Update(points, pose) with `d_xyz` already resident in HBM (packed xyz doubles): used by kicp_register_frame
 int kicp_map_update_pose_packed(kicp_map *m, const double *d_xyz, int64_t n, const double pose[7]);
+// defined in kicp_align.cu: frees the map's alignment scratch (kicp_map_destroy)
+void kicp_align_scratch_free(kicp_map *m);
 // defined in kicp_map.cu: KICP_ERR_INVALID, with kicp_last_error "fn: why"
 int kicp_invalid(const char *fn, const char *why);
 // defined in kicp_frontend.cu: the checks of a device cloud in kicp_frame_input's layout (kicp_*_device) that need no device: n, data,

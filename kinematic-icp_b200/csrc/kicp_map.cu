@@ -420,6 +420,7 @@ extern "C" int kicp_map_destroy(kicp_map *m) {
     cudaFree(m->d_corr_part), cudaFree(m->d_corr_stats), cudaFree(m->d_corr_inl);
     map_live_free(m);
     pose_scratch_free(m);
+    kicp_align_scratch_free(m);
     delete m;
     return KICP_OK;
 }

@@ -23,7 +23,7 @@ __all__ = ["Context", "VoxelHashMap", "Scan", "KinematicRegistration", "KicpErro
            "RegisterFrame", "StageFrame", "StageLaserScan", "RegisterStagedFrame", "StagedFrame", "frame_clouds_f32",
            "frame_clouds_device", "PointCloudSensor", "LaserScanSensor", "StageSensors", "StagedSensors", "RegisterStagedSensors",
            "RegisterStagedFrameSegments", "RegisterStagedSensorsSegments", "deskew_segments", "CorrespondenceStats",
-           "frame_correspondences", "frame_correspondences_device", "PoseHypothesis"]
+           "frame_correspondences", "frame_correspondences_device", "PoseHypothesis", "PlanarAlignment"]
 
 
 class CorrespondenceStats(NamedTuple):
@@ -59,6 +59,28 @@ class PoseHypothesis(NamedTuple):
     def from_c(cls, h):
         return cls(np.array(h.pose[:]), tuple(h.offset), tuple(h.lattice), int(h.level), int(h.n_inliers), float(h.fitness),
                    float(h.inlier_rmse), float(h.sum_sq))
+
+
+class PlanarAlignment(NamedTuple):
+    """kicp_planar_alignment: one start's result of VoxelHashMap.AlignPlanar.  pose (pose7) is the returned pose, status one of
+    KICP_ALIGN_CONVERGED (0), MAX_ITERATIONS (1), NO_CORRESPONDENCES (2), SINGULAR (3), iterations the updates applied, last_step the
+    norm of the last update; the rest is the correspondence report at `pose`: n_inliers, fitness, inlier_rmse, sum_sq, and the
+    unnormalised J^T J (00, 01, 02, 11, 12, 22) and J^T r over (x, y, yaw)."""
+    pose: np.ndarray
+    status: int
+    iterations: int
+    last_step: float
+    n_inliers: int
+    fitness: float
+    inlier_rmse: float
+    sum_sq: float
+    jtj: tuple
+    jtr: tuple
+
+    @classmethod
+    def from_c(cls, a):
+        return cls(np.array(a.pose[:]), int(a.status), int(a.iterations), float(a.last_step), int(a.n_inliers), float(a.fitness),
+                   float(a.inlier_rmse), float(a.sum_sq), tuple(a.jtj), tuple(a.jtr))
 
 
 class Context:
@@ -405,6 +427,32 @@ class VoxelHashMap:
             check(lib().kicp_map_pose_search(self.h, dp(q), len(q), dp(prior), C.byref(p), out, cap, C.byref(n_out),
                                              C.byref(n_scored)), "kicp_map_pose_search")
         return [PoseHypothesis.from_c(out[i]) for i in range(n_out.value)], n_scored.value
+
+    def AlignPlanar(self, points, initial, tau, max_iterations=10, convergence=1e-3, *, stream=None, point_step=0, offsets=(0, 0, 0)):
+        """Gauss-Newton in (x, y, yaw) of `points` (robot base frame) against the map from each starting pose of `initial` (one
+        pose7, or a (k, 7) array-like of 1 to 64 poses, each aligned on its own; kicp_map_align_planar): at most `max_iterations`
+        updates T = T * Delta(dx) over the inliers d < tau, stopping when |dx| < convergence (the defaults are the reference's
+        max_num_iterations and convergence_criterion).  Returns one PlanarAlignment per start, in input order, with the report taken
+        at the returned pose.  One host synchronisation; the map is not modified.
+
+        Device points (taken as AddPoints takes a device cloud) are read on the device (kicp_map_align_planar_device) after the
+        context has waited for `stream`."""
+        starts = np.ascontiguousarray(initial, dtype=np.float64)
+        if starts.ndim not in (1, 2) or starts.shape[-1] != 7:
+            raise ValueError("initial: expected one pose7 or a (k, 7) array of poses")
+        starts = starts.reshape(-1, 7)
+        k = len(starts)
+        p = _capi.PlanarAlignParams(float(tau), float(convergence), int(max_iterations))
+        out = (_capi.PlanarAlignment * max(k, 1))()
+        if _device.is_device(points):
+            d = self._device_points(points, stream, point_step, offsets)
+            check(lib().kicp_map_align_planar_device(self.h, d.ptr, d.n, d.dtype, d.point_step, *d.offsets, dp(starts), k, C.byref(p),
+                                                     out), "kicp_map_align_planar_device")
+        else:
+            _host_only("AlignPlanar", stream=stream, point_step=point_step)
+            q = as_points(points) if len(points) else np.zeros((0, 3))
+            check(lib().kicp_map_align_planar(self.h, dp(q), len(q), dp(starts), k, C.byref(p), out), "kicp_map_align_planar")
+        return [PlanarAlignment.from_c(out[i]) for i in range(k)]
 
 
 def _pinned_corr_stats(ctx):

@@ -67,6 +67,21 @@ class PoseHypothesis(C.Structure):
                 ("n_inliers", C.c_int64), ("fitness", C.c_double), ("inlier_rmse", C.c_double), ("sum_sq", C.c_double)]
 
 
+KICP_ALIGN_CONVERGED, KICP_ALIGN_MAX_ITERATIONS, KICP_ALIGN_NO_CORRESPONDENCES, KICP_ALIGN_SINGULAR = 0, 1, 2, 3
+
+
+class PlanarAlignParams(C.Structure):
+    """kicp_planar_align_params"""
+    _fields_ = [("tau", C.c_double), ("convergence", C.c_double), ("max_iterations", C.c_int32)]
+
+
+class PlanarAlignment(C.Structure):
+    """kicp_planar_alignment"""
+    _fields_ = [("pose", C.c_double * 7), ("status", C.c_int32), ("iterations", C.c_int32), ("last_step", C.c_double),
+                ("n_inliers", C.c_int64), ("fitness", C.c_double), ("inlier_rmse", C.c_double), ("sum_sq", C.c_double),
+                ("jtj", C.c_double * 6), ("jtr", C.c_double * 3)]
+
+
 class FrameInput(C.Structure):
     """kicp_frame_input"""
     _fields_ = [("data", C.c_void_p), ("n", C.c_int64), ("dtype", C.c_int32), ("point_step", C.c_int32), ("offset_x", C.c_int32),
@@ -166,6 +181,9 @@ SYMBOLS = [
     ("kicp_map_pose_search_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp,
                                               C.POINTER(PoseSearchParams), C.POINTER(PoseHypothesis), C.c_int32, C.POINTER(C.c_int32),
                                               C.POINTER(C.c_int64)]),
+    ("kicp_map_align_planar", C.c_int, [_P, c_dp, C.c_int64, c_dp, C.c_int32, C.POINTER(PlanarAlignParams), C.POINTER(PlanarAlignment)]),
+    ("kicp_map_align_planar_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp, C.c_int32,
+                                               C.POINTER(PlanarAlignParams), C.POINTER(PlanarAlignment)]),
     ("kicp_voxel_downsample_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, _P, C.c_int64, C.POINTER(C.c_int64)]),
     ("kicp_preprocess_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, c_dp, c_dp, C.c_double, C.c_double, C.c_int32, _P,
                                          C.c_int64, C.POINTER(C.c_int64)]),
