@@ -464,6 +464,42 @@ int kicp_frame_correspondences(kicp_ctx *ctx, kicp_corr_stats *stats);
  * *n is 0 when the option was off or the frame failed.  Errors: KICP_ERR_INVALID for a null argument, named by kicp_last_error. */
 int kicp_frame_correspondences_device(kicp_ctx *ctx, const double **points, const double **dist, const uint8_t **inlier, int64_t *n);
 
+/* ---- the frame path's map-update policy: whether a frame call (kicp_register_frame, kicp_register_staged_frame, _sensors and the
+ *      _segments variants) ends with the reference's Update(frame_downsample, new_pose), decided on the device within the frame's one
+ *      host synchronisation.  NEVER registers frames against a map that must not change (a map restored with kicp_map_load_voxels);
+ *      GATED inserts only frames whose correspondence report shows that they fit.  The pose, kicp_reg_result, the frame's status, the
+ *      two clouds and the report are those of ALWAYS: the policy decides only whether the map changes. --------------------------- */
+#define KICP_MAP_UPDATE_ALWAYS 0 /* default: Update after every frame whose registration ended KICP_OK (the reference's behaviour) */
+#define KICP_MAP_UPDATE_NEVER 1  /* register against the map as it is: never insert, never evict */
+#define KICP_MAP_UPDATE_GATED 2  /* Update only when the frame's correspondence report passes the thresholds below */
+typedef struct kicp_map_update_policy {
+    int32_t mode;            /* KICP_MAP_UPDATE_* */
+    int64_t min_inliers;     /* GATED: n_inliers >= min_inliers (>= 0) */
+    double min_fitness;      /* GATED: fitness >= min_fitness (in [0, 1]) */
+    double max_inlier_rmse;  /* GATED: inlier_rmse <= max_inlier_rmse (> 0; +inf allowed) */
+} kicp_map_update_policy;
+/* The policy of every later frame call on the context (default {ALWAYS, 0, 0.0, +inf}); the thresholds are ignored outside GATED.
+ * The outcome of a frame, in order: NEVER gives KICP_FRAME_UPDATE_SKIPPED; a registration status other than KICP_OK gives
+ * NO_CORRESPONDENCES; ALWAYS gives APPLIED; GATED gives APPLIED when the map held no points when the frame began (else no map could
+ * ever be built under a gate: the first frame has fitness 0), or when st.n_inliers >= min_inliers, st.fitness >= min_fitness and
+ * st.inlier_rmse <= max_inlier_rmse, where st is the kicp_corr_stats kicp_frame_correspondences returns for that frame, bit for bit;
+ * REJECTED otherwise.  GATED evaluates the report even with option "correspondences" 0 (two more launches, and the report is readable
+ * as if the option were on) and adds one single-thread gate launch; NEVER drops the map's launches.  With option "frame_sync" 1 (or
+ * caller buffers smaller than the frame) the host applies the same rule to the report it has read back.  GATED applies the full Update,
+ * eviction included: it protects a live map; a prior map wider than max_distance is kept only by NEVER.
+ * Errors: KICP_ERR_INVALID, with kicp_last_error naming the field, for a null argument, a mode outside 0..2, min_inliers < 0, a
+ * min_fitness that is NaN or outside [0, 1], or a max_inlier_rmse that is NaN or not > 0; the previous policy is kept. */
+int kicp_ctx_set_map_update(kicp_ctx *ctx, const kicp_map_update_policy *policy);
+#define KICP_FRAME_UPDATE_APPLIED 0            /* the map was updated with the frame */
+#define KICP_FRAME_UPDATE_NO_CORRESPONDENCES 1 /* NaN pose: the map is untouched, as under every policy */
+#define KICP_FRAME_UPDATE_REJECTED 2           /* GATED, thresholds not met: the map is untouched */
+#define KICP_FRAME_UPDATE_SKIPPED 3            /* NEVER: the map is untouched */
+#define KICP_FRAME_UPDATE_NONE 4               /* no frame call yet, the last one failed, or another front-end call came after it */
+/* The outcome of the last frame call on the context (KICP_FRAME_UPDATE_*), with the report's lifetime: valid after a frame call that
+ * returned KICP_OK or KICP_WARN_NO_CORRESPONDENCES, until the next front-end call.  Not a front-end call.  Errors: KICP_ERR_INVALID for
+ * a null argument, named by kicp_last_error. */
+int kicp_frame_map_update(kicp_ctx *ctx, int32_t *outcome);
+
 /* ---- the same frame in two steps, for a caller that needs the sweep's time range before it has the relative odometry (the
  *      online server: ProcessTimestamps -> wheel-odometry lookup over [begin, end] -> RegisterFrame,
  *      ros/.../server/LidarOdometryServer.cpp:186-210). ---------------------------------------------------------------- */

@@ -247,6 +247,14 @@ kicp_corr_stats KinematicICP::LastCorrespondenceStats() const {
 void KinematicICP::SetCorrespondences(bool on) {
     kicp::check(kicp_ctx_set_option(kicp::default_context(), "correspondences", on ? 1 : 0), "kicp_ctx_set_option");
 }
+void KinematicICP::SetMapUpdate(const kicp_map_update_policy &policy) {
+    kicp::check(kicp_ctx_set_map_update(kicp::default_context(), &policy), "kicp_ctx_set_map_update");
+}
+int32_t KinematicICP::LastMapUpdate() const {
+    int32_t outcome = KICP_FRAME_UPDATE_NONE;
+    kicp::check(kicp_frame_map_update(kicp::default_context(), &outcome), "kicp_frame_map_update");
+    return outcome;
+}
 
 // the two clouds of the last frame, built in one pass each from the library's pinned staging
 KinematicICP::Vector3dVectorTuple KinematicICP::StagedClouds() {

@@ -145,6 +145,12 @@ public:
     // none).  SetCorrespondences switches the report for the process-wide context, as KICP_CORRESPONDENCES does at its creation.
     kicp_corr_stats LastCorrespondenceStats() const;
     static void SetCorrespondences(bool on);
+    // Extension: the map-update policy of the process-wide context (kicp_ctx_set_map_update): ALWAYS (the reference's Update after every
+    // frame), NEVER (register against the local map as it is, e.g. one restored with VoxelMap().load_voxels) or GATED (update only
+    // when the frame's correspondence report passes the thresholds).  LastMapUpdate returns kicp_frame_map_update of that context: the
+    // KICP_FRAME_UPDATE_* outcome of the last frame registered on it by any KinematicICP.  Both throw on an error the C call returns.
+    static void SetMapUpdate(const kicp_map_update_policy &policy);
+    int32_t LastMapUpdate() const;
 
     void SetPose(const Sophus::SE3d &pose);  // also clears the map and the threshold statistics (KinematicICP.hpp:85-89)
 

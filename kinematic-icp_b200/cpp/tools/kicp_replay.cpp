@@ -6,7 +6,8 @@
 //
 //   kicp_replay drive.kseq out.tum [--deskew 0|1] [--voxel-size v] [--max-range r] [--min-range r] [--repeat k] [--pageable]
 //               [--host-stamps] [--device-input] [--publish host|device|live] [--publish-digest FILE] [--downsample-order 0|1]
-//               [--correspondences FILE]
+//               [--correspondences FILE] [--map-update always|never|gated] [--min-inliers k] [--min-fitness f]
+//               [--max-inlier-rmse r] [--load-map FILE] [--save-map FILE]
 //
 // .kseq, little endian:  char magic[8] = "KSEQ1\0\0\0"; int32 n_frames; int32 reserved; double lidar_to_base[7]; double start_pose[7];
 //   per frame: int32 n_points; int32 has_stamps; double header_stamp; double relative_odometry[7]; float xyz[3 n]; double stamps[n] (if has_stamps)
@@ -38,6 +39,15 @@
 // registration source at the returned pose against the local map before the frame's update):
 //   stamp, n_points, n_inliers, fitness, inlier_rmse, JTJ00, JTJ01, JTJ11, JTr0, JTr1
 // the stamp as in the TUM file, the doubles with 17 significant digits (they read back to the same bits), no header line.
+// --map-update sets the default context's map-update policy (kicp.h kicp_ctx_set_map_update; KinematicICP::SetMapUpdate): always (the
+// reference's Update after every frame, default), never (register every frame against the map as it is) or gated (update only when
+// the frame's correspondence report passes --min-inliers k (default 0), --min-fitness f (default 0) and --max-inlier-rmse r (default
+// inf), which are accepted only with gated).  --load-map FILE loads a map file (kicp/map_file.hpp, written by --save-map) into the
+// pipeline's map before the first frame of every repetition; its voxel size and max_points_per_voxel must be the replay's.  The drive
+// must start where the map's run started: the pipeline's start pose is the drive's.  --save-map FILE writes the map after the last
+// repetition.  "Map once, localise later" is a --save-map run, then --load-map with --map-update never.  With any of these options
+// the JSON line also reports the policy ("map_update") and how many frames of the last repetition had each outcome
+// ("map_update_outcomes", KinematicICP::LastMapUpdate); without them the line is as before.
 //
 // Version 3, magic "KSEQ3\0\0\0", carries several message streams ("slots", 1..KICP_MAX_SENSORS: PointCloud2 records or 2D LaserScans,
 // each with its extrinsic) and the wheel odometry either as one relative motion or as poses sampled during the sweep:
@@ -68,6 +78,7 @@
 #include <algorithm>
 #include <array>
 #include <chrono>
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -82,6 +93,7 @@
 
 #include "kicp/facade_pipeline.hpp"
 #include "kicp/kseq.hpp"
+#include "kicp/map_file.hpp"
 #include "kicp/runtime.hpp"
 #include "kicp/tum.hpp"
 
@@ -213,7 +225,8 @@ int main(int argc, char **argv) {
     if (argc < 3) {
         std::fprintf(stderr, "usage: %s drive.kseq out.tum [--deskew 0|1] [--voxel-size v] [--max-range r] [--min-range r] [--repeat k] [--pageable] "
                      "[--host-stamps] [--device-input] [--publish host|device|live] [--publish-digest FILE] [--downsample-order 0|1] "
-                     "[--correspondences FILE]\n", argv[0]);
+                     "[--correspondences FILE] [--map-update always|never|gated] [--min-inliers k] [--min-fitness f] [--max-inlier-rmse r] "
+                     "[--load-map FILE] [--save-map FILE]\n", argv[0]);
         return 2;
     }
     kinematic_icp::pipeline::Config config;  // the reference's defaults (pipeline/KinematicICP.hpp:38-60)
@@ -222,6 +235,10 @@ int main(int argc, char **argv) {
     bool pinned = true, host_stamps = false, device_input = false;
     std::string publish = "none", digest_path, corr_path;
     int downsample_order = -1;  // -1: leave the default context's option as it is
+    std::string map_update = "always", load_map_path, save_map_path;
+    kicp_map_update_policy policy{KICP_MAP_UPDATE_ALWAYS, 0, 0.0, HUGE_VAL};
+    bool thresholds = false;  // a --min-* / --max-inlier-rmse option was given (only with --map-update gated)
+    bool map_options = false;  // any of --map-update, the thresholds, --load-map, --save-map: the JSON line reports the outcomes
     for (int i = 3; i < argc; ++i) {
         const std::string a = argv[i];
         auto value = [&](const char *name) -> const char * {
@@ -240,6 +257,12 @@ int main(int argc, char **argv) {
             else if (a == "--publish") publish = value("--publish");
             else if (a == "--publish-digest") digest_path = value("--publish-digest");
             else if (a == "--correspondences") corr_path = value("--correspondences");
+            else if (a == "--map-update") map_update = value("--map-update"), map_options = true;
+            else if (a == "--min-inliers") policy.min_inliers = std::atoll(value("--min-inliers")), thresholds = true;
+            else if (a == "--min-fitness") policy.min_fitness = std::atof(value("--min-fitness")), thresholds = true;
+            else if (a == "--max-inlier-rmse") policy.max_inlier_rmse = std::atof(value("--max-inlier-rmse")), thresholds = true;
+            else if (a == "--load-map") load_map_path = value("--load-map"), map_options = true;
+            else if (a == "--save-map") save_map_path = value("--save-map"), map_options = true;
             else if (a == "--downsample-order") {
                 const std::string v = value("--downsample-order");
                 if (v != "0" && v != "1") throw std::runtime_error("--downsample-order takes 0 or 1");
@@ -251,6 +274,16 @@ int main(int argc, char **argv) {
             return 2;
         }
     }
+    if (map_update != "always" && map_update != "never" && map_update != "gated") {
+        std::fprintf(stderr, "kicp_replay: --map-update takes always, never or gated\n");
+        return 2;
+    }
+    if (thresholds && map_update != "gated") {
+        std::fprintf(stderr, "kicp_replay: --min-inliers, --min-fitness and --max-inlier-rmse need --map-update gated\n");
+        return 2;
+    }
+    map_options = map_options || thresholds;
+    policy.mode = map_update == "never" ? KICP_MAP_UPDATE_NEVER : map_update == "gated" ? KICP_MAP_UPDATE_GATED : KICP_MAP_UPDATE_ALWAYS;
     if (publish != "none" && publish != "host" && publish != "device" && publish != "live") {
         std::fprintf(stderr, "kicp_replay: --publish takes host, device or live\n");
         return 2;
@@ -274,6 +307,15 @@ int main(int argc, char **argv) {
         if (downsample_order >= 0)
             kicp::check(kicp_ctx_set_option(kicp::default_context(), "downsample_order", downsample_order), "--downsample-order");
         if (!corr_path.empty()) kinematic_icp::pipeline::KinematicICP::SetCorrespondences(true);
+        if (map_options) kinematic_icp::pipeline::KinematicICP::SetMapUpdate(policy);  // a threshold out of range throws, naming the field
+        kicp::MapFile prior;  // --load-map
+        if (!load_map_path.empty()) {
+            prior = kicp::read_map_file(load_map_path);
+            if (prior.voxel_size != config.voxel_size || prior.max_points_per_voxel != config.max_points_per_voxel)
+                throw std::runtime_error(load_map_path + ": voxel size " + std::to_string(prior.voxel_size) + " and max_points_per_voxel " +
+                                         std::to_string(prior.max_points_per_voxel) + " differ from the replay's " +
+                                         std::to_string(config.voxel_size) + " and " + std::to_string(config.max_points_per_voxel));
+        }
         bool v2 = false;
         double l2b[7], start[7];
         std::vector<Frame> frames;  // KSEQ1 / KSEQ2
@@ -341,10 +383,16 @@ int main(int argc, char **argv) {
         int64_t map_points = 0;  // the local map's size after the last frame
         int64_t live_written = 0, live_records = 0;  // --publish live, last repetition: records written, and published, over all frames
         double map_seconds = 0.0;  // --publish, last repetition: time spent publishing the local map
+        int64_t outcomes[KICP_FRAME_UPDATE_NONE + 1] = {};  // frames of the last repetition per KICP_FRAME_UPDATE_* outcome
         std::vector<double> rep_seconds;  // every repetition's wall time (a 24-frame drive lasts milliseconds: one hiccup halves a single figure)
         for (int rep = 0; rep < repeat; ++rep) {  // --repeat: the same drive again on a fresh pipeline (the last run is the one written)
             kinematic_icp::pipeline::KinematicICP pipeline(config);
-            pipeline.SetPose(kicp::from_pose7(start));
+            pipeline.SetPose(kicp::from_pose7(start));  // (clears the map: the prior map is loaded after it)
+            if (!load_map_path.empty())
+                kicp::check(kicp_map_load_voxels(pipeline.VoxelMap().handle_, prior.keys.data(), prior.counts.data(), prior.points.data(),
+                                                 prior.num_voxels()),
+                            "kicp_map_load_voxels");
+            for (int64_t &o : outcomes) o = 0;
             poses.clear();
             poses.reserve((size_t)n_frames);
             digests.clear();
@@ -353,6 +401,7 @@ int main(int argc, char **argv) {
             auto frame_done = [&](double stamp) {
                 poses.emplace_back(stamp, pipeline.pose());
                 if (!corr_path.empty()) corr.push_back(pipeline.LastCorrespondenceStats());
+                ++outcomes[pipeline.LastMapUpdate()];
             };
             live_written = live_records = 0;
             map_seconds = 0.0;
@@ -449,6 +498,17 @@ int main(int argc, char **argv) {
             seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
             rep_seconds.push_back(seconds);
             kicp::check(kicp_map_num_points(pipeline.VoxelMap().handle_, &map_points), "kicp_map_num_points");
+            if (!save_map_path.empty() && rep == repeat - 1) {  // the map after the last repetition, as kicp_map_export_voxels gives it
+                kicp_map *h = pipeline.VoxelMap().handle_;
+                kicp::MapFile out;
+                out.voxel_size = config.voxel_size, out.max_points_per_voxel = config.max_points_per_voxel;
+                int64_t nv = 0, np = 0;
+                kicp::check(kicp_map_num_voxels(h, &nv), "kicp_map_num_voxels");
+                out.keys.resize(3 * (size_t)nv), out.counts.resize((size_t)nv), out.points.resize(3 * (size_t)map_points);
+                kicp::check(kicp_map_export_voxels(h, out.keys.data(), out.counts.data(), out.points.data(), nv, map_points, &nv, &np),
+                            "kicp_map_export_voxels");
+                kicp::write_map_file(save_map_path, out);
+            }
         }
         // the fastest repetition after the first (which also pays for allocations); the last one stays the headline of this line
         double best = seconds;
@@ -488,6 +548,15 @@ int main(int argc, char **argv) {
             char buf[128];
             std::snprintf(buf, sizeof(buf), ", \"live_written_per_frame\": %.1f, \"live_map_records_per_frame\": %.1f",
                           n_frames ? (double)live_written / n_frames : 0.0, n_frames ? (double)live_records / n_frames : 0.0);
+            live += buf;
+        }
+        if (map_options) {  // the map-update policy and the outcomes of the last repetition's frames
+            char buf[256];
+            std::snprintf(buf, sizeof(buf), ", \"map_update\": \"%s\", \"map_update_outcomes\": {\"applied\": %lld, \"no_correspondences\": %lld, "
+                          "\"rejected\": %lld, \"skipped\": %lld, \"none\": %lld}", map_update.c_str(),
+                          (long long)outcomes[KICP_FRAME_UPDATE_APPLIED], (long long)outcomes[KICP_FRAME_UPDATE_NO_CORRESPONDENCES],
+                          (long long)outcomes[KICP_FRAME_UPDATE_REJECTED], (long long)outcomes[KICP_FRAME_UPDATE_SKIPPED],
+                          (long long)outcomes[KICP_FRAME_UPDATE_NONE]);
             live += buf;
         }
         if (v3) {  // the slots, their kinds, and the odometry samples per frame (0: one motion per frame)

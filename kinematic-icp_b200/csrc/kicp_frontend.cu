@@ -21,6 +21,7 @@ using namespace kicp_dev;
 #include "kicp_downsample_order_kernels.cuh"  // option "downsample_order" 1: the robin_map order of the down-sample
 #include "kicp_sensors_kernels.cuh"  // the multi-sensor frame: the common sweep window and the segmented Preprocess
 #include "kicp_segments_kernels.cuh"  // the piecewise de-skew: per-sensor tables of constant-velocity segments
+#include "kicp_map_update_kernels.cuh"  // the map-update policy: the rule and the gate of KICP_MAP_UPDATE_GATED
 static_assert(kMaxSensors == KICP_MAX_SENSORS, "kicp_sensors_kernels.cuh and kicp.h disagree");
 static_assert(kMaxDeskewSegments == KICP_MAX_DESKEW_SEGMENTS, "kicp_segments_kernels.cuh and kicp.h disagree");
 
@@ -159,6 +160,12 @@ struct Scratch {
     kicp_corr_stats *h_corr = nullptr;
     int64_t corr_cap = 0, corr_n = 0;
     kicp_corr_stats corr = {};
+    // the map-update policy: the last frame's outcome as kicp_frame_map_update returns it (the report's lifetime: NONE after any other
+    // front-end call and a frame that failed), and for GATED in the single-synchronisation order the gate's shadow result block and
+    // outcome word (device, allocated on the first such frame) and the outcome's pinned copy
+    int32_t map_update = KICP_FRAME_UPDATE_NONE;
+    kicp_reg_result *d_shadow = nullptr;
+    int32_t *d_gate = nullptr, *h_gate = nullptr;
     double timing[8] = {0};  // host-side stage times of the last kicp_register_frame, milliseconds (debug export)
     int *first_idx = nullptr, *slot_of = nullptr, *d_count = nullptr;
     int4 *slots = nullptr;
@@ -181,6 +188,7 @@ void release(Scratch &s) {
     cudaFree(s.d_seg_mm), cudaFree(s.d_seg_count), cudaFreeHost(s.h_seg_mm), cudaFreeHost(s.h_seg_count);
     cudaFree(s.d_segs), cudaFreeHost(s.h_segs);
     cudaFree(s.corr_pts), cudaFree(s.corr_dist), cudaFree(s.corr_inl), cudaFreeHost(s.h_corr);
+    cudaFree(s.d_shadow), cudaFree(s.d_gate), cudaFreeHost(s.h_gate);
     if (s.ev_segs) cudaEventDestroy(s.ev_segs);
     s.staged.release();
     if (s.ev_front) cudaEventDestroy(s.ev_front);
@@ -310,6 +318,17 @@ int reserve_corr(Scratch &s) {
     return KICP_OK;
 }
 
+// the gate's buffers (KICP_MAP_UPDATE_GATED, allocated on the first gated frame of the single-synchronisation order); the shadow block
+// starts zeroed, and the gate writes its pose and status before every use
+int reserve_gate(Scratch &s) {
+    if (s.d_shadow) return KICP_OK;
+    KICP_CUDA(cudaMalloc(&s.d_shadow, sizeof(kicp_reg_result)));
+    KICP_CUDA(cudaMemset(s.d_shadow, 0, sizeof(kicp_reg_result)));
+    KICP_CUDA(cudaMalloc(&s.d_gate, sizeof(int32_t)));
+    KICP_CUDA(cudaMallocHost(&s.h_gate, sizeof(int32_t)));
+    return KICP_OK;
+}
+
 // VoxelDownsample of src[0, n) (n = *d_n when given, else n_max) into dst, survivor count to d_count_out; all on the stream:
 // clear the scratch hash, claim a slot per voxel with the smallest input index, select the points that hold their voxel's index.
 // With option "downsample_order" 1 the select writes to s.ro_pts and five more launches put the survivors into the robin_map's bucket
@@ -431,7 +450,7 @@ int open_frontend(kicp_ctx *c, int status, int64_t n) {
     if (c) {
         Scratch &s = scratch(c);
         s.held_n = -1, s.dev_n_frame = s.dev_n_source = 0;
-        s.corr_n = 0, s.corr = kicp_corr_stats{};
+        s.corr_n = 0, s.corr = kicp_corr_stats{}, s.map_update = KICP_FRAME_UPDATE_NONE;
     }
     if (status != KICP_OK) return status;
     KICP_CUDA(cudaSetDevice(c->device));
@@ -630,8 +649,8 @@ struct FrameArgs {
     }
 };
 
-// KinematicICP::RegisterFrame from the frame in s.in[0, n) on: Preprocess, both down-samples, registration, map update, the two
-// clouds.  A frame is ONE host synchronisation (at its end): every later stage reads the survivor counts and the pose from device
+// KinematicICP::RegisterFrame from the frame in s.in[0, n) on: Preprocess, both down-samples, registration, map update (as the
+// context's map-update policy decides, kicp_map_update.h), the two clouds.  A frame is ONE host synchronisation (at its end): every later stage reads the survivor counts and the pose from device
 // memory, and the registration and the staging copies are sized by upper bounds.  The read-back order (read the counts back, size
 // everything exactly) remains for callers whose output buffers might be too small for the worst case — they are owed
 // KICP_ERR_CAPACITY before the map changes — and as option "frame_sync" for A/B measurements.
@@ -644,10 +663,16 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
     const bool stage = (fp->stage_clouds & ~KICP_STAGE_F32) != 0 || a.out_frame || a.out_source;
     const bool stage32 = (fp->stage_clouds & KICP_STAGE_F32) != 0;
     const bool one_sync = n > 0 && !c->frame_sync && (!a.out_frame || a.cap_frame >= n) && (!a.out_source || a.cap_source >= n);
-    const bool corr = c->correspondences != 0;
-    s.corr_n = 0, s.corr = kicp_corr_stats{};
+    // the policy: NEVER enqueues no Update; GATED decides on the report, which it evaluates whatever option "correspondences" says,
+    // and on whether the map held points before the frame (the host mirror is current: every frame call ends with it up to date)
+    const kicp_map_update_policy policy = c->map_update;
+    const bool never = policy.mode == KICP_MAP_UPDATE_NEVER, gated = policy.mode == KICP_MAP_UPDATE_GATED;
+    const bool map_was_empty = map->num_points == 0;
+    const bool corr = c->correspondences != 0 || gated;
+    s.corr_n = 0, s.corr = kicp_corr_stats{}, s.map_update = KICP_FRAME_UPDATE_NONE;
     // the report's buffers are sized before anything of this frame is enqueued: a growth (cudaFree / cudaMalloc) waits for the device
     if (corr) KICP_TRY(reserve_corr(s));
+    if (gated && one_sync) KICP_TRY(reserve_gate(s));
     // the survivor counts of the three stages (12 bytes back, one synchronisation of the stream)
     int counts[3] = {0, 0, 0};
     auto read_counts = [&]() -> int {
@@ -707,9 +732,19 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
                                                   s.corr_dist, s.corr_inl, s.h_corr));
     }
     if (one_sync) {
-        // local_map_.Update(frame_downsample, new_pose) (KinematicICP.cpp:79), pose and count still on the device
-        KICP_TRY(kicp_map_update_pose_async(map, reinterpret_cast<const double *>(s.out2), n, s.d_count + 1, kicp_device_result(c),
-                                            s.h_mapctr));
+        if (!never) {
+            // local_map_.Update(frame_downsample, new_pose) (KinematicICP.cpp:79), pose and count still on the device.  Under GATED the
+            // gate reads the result block and the report's statistics (the bytes copied to s.h_corr above) and hands the map's kernels
+            // a shadow block whose status is KICP_OK only when the update is applied; they leave the map untouched otherwise.
+            const kicp_reg_result *d_res = kicp_device_result(c);
+            if (gated) {
+                k_map_update_gate<<<1, 1, 0, c->stream>>>(d_res, map->d_corr_stats, policy, map_was_empty ? 1 : 0, s.d_shadow, s.d_gate);
+                KICP_CHECK_LAUNCH(c);
+                KICP_CUDA(cudaMemcpyAsync(s.h_gate, s.d_gate, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+                d_res = s.d_shadow;
+            }
+            KICP_TRY(kicp_map_update_pose_async(map, reinterpret_cast<const double *>(s.out2), n, s.d_count + 1, d_res, s.h_mapctr));
+        }
         KICP_TRY(read_counts());  // THE synchronisation of the frame
     } else {
         KICP_CUDA(cudaStreamSynchronize(c->stream));
@@ -719,11 +754,14 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
     for (int k = 0; k < 7; ++k) a.out_pose[k] = r.pose[k];
     if (a.result) *a.result = r;
     int status = r.status;
-    // a NaN pose (zero correspondences, which the reference does not defend against) is reported and leaves the map untouched
+    // a NaN pose (zero correspondences, which the reference does not defend against) is reported and leaves the map untouched; in the
+    // read-back order the host applies the gate's rule to the statistics it has read back
+    const int32_t outcome = one_sync && gated ? *s.h_gate
+                                              : map_update_outcome(policy, r.status, map_was_empty, corr ? *s.h_corr : kicp_corr_stats{});
     if (one_sync) {
-        const int mst = kicp_map_finish_update(map, s.h_mapctr, false);
+        const int mst = never ? KICP_OK : kicp_map_finish_update(map, s.h_mapctr, false);
         if (mst != KICP_OK) status = mst;
-    } else if (status == KICP_OK && counts[1] > 0) {
+    } else if (outcome == KICP_FRAME_UPDATE_APPLIED && counts[1] > 0) {
         status = kicp_map_update_pose_packed(map, reinterpret_cast<const double *>(s.out2), counts[1], r.pose);
     }
     s.timing[3] = ms_since();  // + map update
@@ -733,6 +771,7 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
     if (status == KICP_OK || status == KICP_WARN_NO_CORRESPONDENCES) {
         s.dev_n_frame = counts[0], s.dev_n_source = counts[2], s.dev_f32 = stage32;
         if (corr) s.corr_n = counts[2], s.corr = *s.h_corr;
+        s.map_update = outcome;
     }
     s.timing[4] = ms_since();  // + clouds delivered
     return status;
@@ -1276,6 +1315,30 @@ extern "C" int kicp_frame_correspondences_device(kicp_ctx *c, const double **poi
     const Scratch &s = scratch(c);
     *points = reinterpret_cast<const double *>(s.corr_pts), *dist = s.corr_dist, *inlier = s.corr_inl;
     *n = s.corr_n;
+    return KICP_OK;
+}
+
+// The map-update policy of the frame calls (kicp_map_update.h): checked field by field, the context last; a failing call keeps the
+// previous policy
+extern "C" int kicp_ctx_set_map_update(kicp_ctx *c, const kicp_map_update_policy *policy) {
+    static const char fn[] = "kicp_ctx_set_map_update";
+    if (!policy) return kicp_invalid(fn, "policy: null pointer");
+    const kicp_map_update_policy &p = *policy;
+    if (p.mode < KICP_MAP_UPDATE_ALWAYS || p.mode > KICP_MAP_UPDATE_GATED) return kicp_invalid(fn, "policy->mode: not in 0..2");
+    if (p.min_inliers < 0) return kicp_invalid(fn, "policy->min_inliers: negative");
+    if (!(p.min_fitness >= 0.0 && p.min_fitness <= 1.0)) return kicp_invalid(fn, "policy->min_fitness: not in [0, 1]");
+    if (!(p.max_inlier_rmse > 0.0)) return kicp_invalid(fn, "policy->max_inlier_rmse: not > 0");
+    if (!c) return kicp_invalid(fn, "null context");
+    c->map_update = p;
+    return KICP_OK;
+}
+
+// The map-update outcome of the last frame call; not a front-end call
+extern "C" int kicp_frame_map_update(kicp_ctx *c, int32_t *outcome) {
+    static const char fn[] = "kicp_frame_map_update";
+    if (!outcome) return kicp_invalid(fn, "outcome: null pointer");
+    if (!c) return kicp_invalid(fn, "null context");
+    *outcome = scratch(c).map_update;
     return KICP_OK;
 }
 

@@ -1,6 +1,7 @@
 // Internal definitions shared by the translation units of libkicp_b200.so.  Not installed.
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 #include <string>
@@ -66,6 +67,8 @@ struct kicp_ctx {
     int frame_sync = 0;       // option "frame_sync": 1 = kicp_register_frame reads the survivor counts back mid-frame (legacy order)
     int downsample_order = 0;  // option "downsample_order": 1 = VoxelDownsample emits the robin_map's bucket order (kicp_frontend.cu)
     int correspondences = 0;   // option "correspondences": 1 = the frame calls evaluate the source at the returned pose (kicp_frontend.cu)
+    // kicp_ctx_set_map_update: whether the frame calls end with the map's Update (kicp_frontend.cu)
+    kicp_map_update_policy map_update = {KICP_MAP_UPDATE_ALWAYS, 0, 0.0, INFINITY};
     int overlap_upload = 1;
     // the registration's device state, neighbour cache, upload flags and profiling records (kicp_register_api.cu owns the type)
     struct RegScratch *reg = nullptr;

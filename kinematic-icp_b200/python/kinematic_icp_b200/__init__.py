@@ -9,6 +9,7 @@ Poses are pose7 = [qx, qy, qz, qw, tx, ty, tz] (Sophus::SE3d's two members); poi
 Everything runs on the GPU through libkicp_b200.so (include/kicp.h); there is no CPU fallback.
 """
 import ctypes as C
+import math
 from typing import NamedTuple
 
 import numpy as np
@@ -23,7 +24,7 @@ __all__ = ["Context", "VoxelHashMap", "Scan", "KinematicRegistration", "KicpErro
            "RegisterFrame", "StageFrame", "StageLaserScan", "RegisterStagedFrame", "StagedFrame", "frame_clouds_f32",
            "frame_clouds_device", "PointCloudSensor", "LaserScanSensor", "StageSensors", "StagedSensors", "RegisterStagedSensors",
            "RegisterStagedFrameSegments", "RegisterStagedSensorsSegments", "deskew_segments", "CorrespondenceStats",
-           "frame_correspondences", "frame_correspondences_device", "PoseHypothesis", "PlanarAlignment"]
+           "frame_correspondences", "frame_correspondences_device", "PoseHypothesis", "PlanarAlignment", "frame_map_update"]
 
 
 class CorrespondenceStats(NamedTuple):
@@ -104,6 +105,14 @@ class Context:
 
     def set_option(self, name, value):
         check(lib().kicp_ctx_set_option(self.h, name.encode(), int(value)), "kicp_ctx_set_option")
+
+    def set_map_update(self, mode, *, min_inliers=0, min_fitness=0.0, max_inlier_rmse=math.inf):
+        """kicp_ctx_set_map_update: whether every later frame call on the context ends with the map's Update.  mode is
+        _capi.KICP_MAP_UPDATE_ALWAYS (0, default), NEVER (1: register against the map as it is) or GATED (2: update only when the frame's
+        correspondence report has n_inliers >= min_inliers, fitness >= min_fitness and inlier_rmse <= max_inlier_rmse, or the map was
+        empty).  frame_map_update(ctx) tells what the last frame did."""
+        p = _capi.MapUpdatePolicy(int(mode), int(min_inliers), float(min_fitness), float(max_inlier_rmse))
+        check(lib().kicp_ctx_set_map_update(self.h, C.byref(p)), "kicp_ctx_set_map_update")
 
     def wait_stream(self, stream):
         """kicp_ctx_wait_stream: the context's later work waits for everything enqueued on `stream` (a cudaStream_t int) so far."""
@@ -472,6 +481,15 @@ def frame_correspondences(ctx):
     st = _capi.CorrStats()
     check(lib().kicp_frame_correspondences(ctx.h, C.byref(st)), "kicp_frame_correspondences")
     return CorrespondenceStats.from_c(st)
+
+
+def frame_map_update(ctx):
+    """The map-update outcome of the last frame call on `ctx` (kicp_frame_map_update): _capi.KICP_FRAME_UPDATE_APPLIED (0),
+    NO_CORRESPONDENCES (1), REJECTED (2), SKIPPED (3), or NONE (4) before the first frame, after a frame that failed, and after any other
+    front-end call."""
+    o = C.c_int32()
+    check(lib().kicp_frame_map_update(ctx.h, C.byref(o)), "kicp_frame_map_update")
+    return int(o.value)
 
 
 def frame_correspondences_device(ctx):

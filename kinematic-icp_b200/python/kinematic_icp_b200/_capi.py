@@ -82,6 +82,16 @@ class PlanarAlignment(C.Structure):
                 ("jtj", C.c_double * 6), ("jtr", C.c_double * 3)]
 
 
+KICP_MAP_UPDATE_ALWAYS, KICP_MAP_UPDATE_NEVER, KICP_MAP_UPDATE_GATED = 0, 1, 2
+KICP_FRAME_UPDATE_APPLIED, KICP_FRAME_UPDATE_NO_CORRESPONDENCES, KICP_FRAME_UPDATE_REJECTED, KICP_FRAME_UPDATE_SKIPPED, \
+    KICP_FRAME_UPDATE_NONE = 0, 1, 2, 3, 4
+
+
+class MapUpdatePolicy(C.Structure):
+    """kicp_map_update_policy"""
+    _fields_ = [("mode", C.c_int32), ("min_inliers", C.c_int64), ("min_fitness", C.c_double), ("max_inlier_rmse", C.c_double)]
+
+
 class FrameInput(C.Structure):
     """kicp_frame_input"""
     _fields_ = [("data", C.c_void_p), ("n", C.c_int64), ("dtype", C.c_int32), ("point_step", C.c_int32), ("offset_x", C.c_int32),
@@ -210,6 +220,8 @@ SYMBOLS = [
     ("kicp_frame_clouds_device", C.c_int, [_P, C.c_int32, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(_P), C.POINTER(C.c_int64)]),
     ("kicp_frame_correspondences", C.c_int, [_P, C.POINTER(CorrStats)]),
     ("kicp_frame_correspondences_device", C.c_int, [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_int64)]),
+    ("kicp_ctx_set_map_update", C.c_int, [_P, C.POINTER(MapUpdatePolicy)]),
+    ("kicp_frame_map_update", C.c_int, [_P, C.POINTER(C.c_int32)]),
     ("kicp_frame_stage", C.c_int, [_P, C.POINTER(FrameInput), C.c_int32, C.c_int32, c_dp, C.POINTER(C.c_int64)]),
     ("kicp_frame_stage_device", C.c_int, [_P, C.POINTER(FrameInput), C.c_int32, C.c_int32, c_dp, C.POINTER(C.c_int64)]),
     ("kicp_register_staged_frame", C.c_int, [_P, c_dp, c_dp, c_dp, c_dp, C.c_double, C.POINTER(FrameParams), c_dp, c_dp, C.c_int64,
