@@ -192,6 +192,38 @@ int kicp_map_export_voxels(kicp_map *map, int32_t *keys, int32_t *counts, double
 /* Bulk load of a voxel-grouped map (replaces the content): the inverse of kicp_map_export_voxels. */
 int kicp_map_load_voxels(kicp_map *map, const int32_t *keys, const int32_t *counts, const double *points,
                          int64_t num_voxels);
+/* ---- a frozen prior inside the map: a map has P prior voxels (0 by default), the first P voxels in its block order (the order of
+ *      kicp_map_export_voxels and kicp_map_pointcloud).  Every reader (registration, nearest, correspondences, pose search, planar
+ *      alignment, the exports) sees one map: the prior voxels followed by the live ones.
+ *   - Prior voxels are read-only: while frozen their keys, counts and point bytes do not change, and they stay at positions [0, P).
+ *   - Insertion: every AddPoints (host and _device variants, both Updates, the frame path's Update in both synchronisation orders)
+ *     drops a point whose voxel key is a prior voxel's; every other point follows the reference's rule, which looks only inside the
+ *     point's own voxel.  The live voxels are therefore exactly the map the same calls build from an empty map, fed only the points
+ *     that were not dropped.
+ *   - Eviction: prior voxels never die; live voxels die by the reference's rule (first point >= max_distance from the origin).
+ *   - The frame path's map-update policy is unchanged: NEVER skips the whole Update, ALWAYS and GATED apply it to the live voxels, and
+ *     GATED's "the map held no points" is about the whole map.
+ *   - kicp_map_clear and kicp_map_load_voxels reset P to 0 ("load, then freeze" is two calls); so does the facade's SetPose, which
+ *     clears the map as the reference does.  A map that never freezes runs exactly the code, launches and bytes it ran before.
+ *   - Cost while frozen: an Update compacts and re-inserts only the live voxels, plus one device copy of a snapshot of the prior's
+ *     hash table (16 bytes a slot, 4 to 8 slots per voxel of capacity); freezing copies the prior once into the spare block arrays.
+ * kicp_map_freeze: every voxel now in the map becomes prior (P = number of voxels); a second freeze also takes in the live voxels
+ * added since.  kicp_map_thaw: P = 0, the voxels stay as ordinary ones (the next eviction may remove them).  Both synchronise.
+ * kicp_map_pointcloud_f32_live still diffs the whole map.  Errors: KICP_ERR_INVALID for a null argument, named by kicp_last_error. */
+int kicp_map_freeze(kicp_map *map);
+int kicp_map_thaw(kicp_map *map);
+/* the prior's voxel and point counts (0, 0 when nothing is frozen) */
+int kicp_map_prior_size(kicp_map *map, int64_t *voxels, int64_t *points);
+#define KICP_MAP_LAYER_ALL 0   /* every voxel: kicp_map_pointcloud's points */
+#define KICP_MAP_LAYER_PRIOR 1 /* the frozen prior voxels [0, P) */
+#define KICP_MAP_LAYER_LIVE 2  /* the voxels after them */
+/* kicp_map_pointcloud (dtype KICP_DTYPE_F64) or kicp_map_pointcloud_f32 (KICP_DTYPE_F32) of one layer: ALL is PRIOR followed by LIVE,
+ * byte for byte.  A node that localises on a prior publishes PRIOR once and LIVE every frame.  *n receives the layer's point count.
+ * The _device_async form packs into device memory as kicp_map_pointcloud_device_async does.  Errors: KICP_ERR_INVALID for a null
+ * argument, a layer or dtype outside the values above, or (device) `out` that is not such memory, named by kicp_last_error;
+ * KICP_ERR_CAPACITY when cap < *n (nothing copied). */
+int kicp_map_pointcloud_layer(kicp_map *map, int32_t layer, int32_t dtype, void *out, int64_t cap, int64_t *n);
+int kicp_map_pointcloud_layer_device_async(kicp_map *map, int32_t layer, int32_t dtype, void *out, int64_t cap, int64_t *n);
 /* GetClosestNeighbor(query) for n queries: (closest point, distance); (0,0,0), DBL_MAX when nothing is found. */
 int kicp_map_nearest(kicp_map *map, const double *queries, int64_t n, double *out_points, double *out_dist);
 /* ---- the map operators on clouds in device memory.  `data` holds n points of device memory of the context's device in the layout of
@@ -486,7 +518,8 @@ typedef struct kicp_map_update_policy {
  * REJECTED otherwise.  GATED evaluates the report even with option "correspondences" 0 (two more launches, and the report is readable
  * as if the option were on) and adds one single-thread gate launch; NEVER drops the map's launches.  With option "frame_sync" 1 (or
  * caller buffers smaller than the frame) the host applies the same rule to the report it has read back.  GATED applies the full Update,
- * eviction included: it protects a live map; a prior map wider than max_distance is kept only by NEVER.
+ * eviction included: it protects a live map; a prior map wider than max_distance is kept by NEVER, or by freezing it
+ * (kicp_map_freeze), after which ALWAYS and GATED update only the live voxels beside it.
  * Errors: KICP_ERR_INVALID, with kicp_last_error naming the field, for a null argument, a mode outside 0..2, min_inliers < 0, a
  * min_fitness that is NaN or outside [0, 1], or a max_inlier_rmse that is NaN or not > 0; the previous policy is kept. */
 int kicp_ctx_set_map_update(kicp_ctx *ctx, const kicp_map_update_policy *policy);

@@ -80,6 +80,31 @@ struct VoxelHashMap {
         if (n > 0) kicp::check(kicp_map_pointcloud(handle_, out.front().data(), n, &n), "kicp_map_pointcloud");
         return out;
     }
+    // A frozen prior inside the map (kicp_map_freeze): every voxel now in the map becomes read-only and is never evicted; later
+    // Updates build the live layer beside it.  Clear() (and so KinematicICP::SetPose) and load_voxels remove the prior too.
+    void Freeze() { kicp::check(kicp_map_freeze(handle_), "kicp_map_freeze"); }
+    void Thaw() { kicp::check(kicp_map_thaw(handle_), "kicp_map_thaw"); }
+    int64_t PriorVoxels() const {
+        int64_t v = 0, n = 0;
+        kicp::check(kicp_map_prior_size(handle_, &v, &n), "kicp_map_prior_size");
+        return v;
+    }
+    int64_t PriorPoints() const {
+        int64_t v = 0, n = 0;
+        kicp::check(kicp_map_prior_size(handle_, &v, &n), "kicp_map_prior_size");
+        return n;
+    }
+    // Pointcloud() of one layer (KICP_MAP_LAYER_ALL, _PRIOR or _LIVE): ALL is PRIOR followed by LIVE
+    std::vector<Eigen::Vector3d> Pointcloud(int32_t layer) const {
+        int64_t n = 0, total = 0;
+        kicp::check(kicp_map_num_points(handle_, &total), "kicp_map_num_points");
+        const int64_t prior = PriorPoints();
+        n = layer == KICP_MAP_LAYER_PRIOR ? prior : layer == KICP_MAP_LAYER_LIVE ? total - prior : total;
+        std::vector<Eigen::Vector3d> out(static_cast<size_t>(n));
+        if (n == 0) kicp::check(kicp_map_pointcloud_layer(handle_, layer, KICP_DTYPE_F64, nullptr, 0, &n), "kicp_map_pointcloud_layer");
+        if (n > 0) kicp::check(kicp_map_pointcloud_layer(handle_, layer, KICP_DTYPE_F64, out.front().data(), n, &n), "kicp_map_pointcloud_layer");
+        return out;
+    }
     std::tuple<Eigen::Vector3d, double> GetClosestNeighbor(const Eigen::Vector3d &query) const {
         Eigen::Vector3d p;
         double d = 0.0;

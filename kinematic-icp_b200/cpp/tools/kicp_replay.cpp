@@ -7,7 +7,7 @@
 //   kicp_replay drive.kseq out.tum [--deskew 0|1] [--voxel-size v] [--max-range r] [--min-range r] [--repeat k] [--pageable]
 //               [--host-stamps] [--device-input] [--publish host|device|live] [--publish-digest FILE] [--downsample-order 0|1]
 //               [--correspondences FILE] [--map-update always|never|gated] [--min-inliers k] [--min-fitness f]
-//               [--max-inlier-rmse r] [--load-map FILE] [--save-map FILE]
+//               [--max-inlier-rmse r] [--load-map FILE] [--freeze-prior] [--save-map FILE]
 //
 // .kseq, little endian:  char magic[8] = "KSEQ1\0\0\0"; int32 n_frames; int32 reserved; double lidar_to_base[7]; double start_pose[7];
 //   per frame: int32 n_points; int32 has_stamps; double header_stamp; double relative_odometry[7]; float xyz[3 n]; double stamps[n] (if has_stamps)
@@ -47,7 +47,11 @@
 // must start where the map's run started: the pipeline's start pose is the drive's.  --save-map FILE writes the map after the last
 // repetition.  "Map once, localise later" is a --save-map run, then --load-map with --map-update never.  With any of these options
 // the JSON line also reports the policy ("map_update") and how many frames of the last repetition had each outcome
-// ("map_update_outcomes", KinematicICP::LastMapUpdate); without them the line is as before.
+// ("map_update_outcomes", KinematicICP::LastMapUpdate); without them the line is as before.  --freeze-prior (only with --load-map)
+// freezes the loaded map (kicp_map_freeze): its voxels are never evicted or written into, and the frames' Updates build a live layer
+// beside it.  "Localise on a prior map that keeps learning" is --load-map FILE --freeze-prior --map-update always (or gated).  The JSON
+// line then also reports the prior's and the live layer's voxel and point counts at the end of the last repetition ("prior_voxels",
+// "prior_points", "live_voxels", "live_points").
 //
 // Version 3, magic "KSEQ3\0\0\0", carries several message streams ("slots", 1..KICP_MAX_SENSORS: PointCloud2 records or 2D LaserScans,
 // each with its extrinsic) and the wheel odometry either as one relative motion or as poses sampled during the sweep:
@@ -226,7 +230,7 @@ int main(int argc, char **argv) {
         std::fprintf(stderr, "usage: %s drive.kseq out.tum [--deskew 0|1] [--voxel-size v] [--max-range r] [--min-range r] [--repeat k] [--pageable] "
                      "[--host-stamps] [--device-input] [--publish host|device|live] [--publish-digest FILE] [--downsample-order 0|1] "
                      "[--correspondences FILE] [--map-update always|never|gated] [--min-inliers k] [--min-fitness f] [--max-inlier-rmse r] "
-                     "[--load-map FILE] [--save-map FILE]\n", argv[0]);
+                     "[--load-map FILE] [--freeze-prior] [--save-map FILE]\n", argv[0]);
         return 2;
     }
     kinematic_icp::pipeline::Config config;  // the reference's defaults (pipeline/KinematicICP.hpp:38-60)
@@ -237,6 +241,7 @@ int main(int argc, char **argv) {
     int downsample_order = -1;  // -1: leave the default context's option as it is
     std::string map_update = "always", load_map_path, save_map_path;
     kicp_map_update_policy policy{KICP_MAP_UPDATE_ALWAYS, 0, 0.0, HUGE_VAL};
+    bool freeze_prior = false;  // --freeze-prior: freeze the map --load-map loaded
     bool thresholds = false;  // a --min-* / --max-inlier-rmse option was given (only with --map-update gated)
     bool map_options = false;  // any of --map-update, the thresholds, --load-map, --save-map: the JSON line reports the outcomes
     for (int i = 3; i < argc; ++i) {
@@ -263,6 +268,7 @@ int main(int argc, char **argv) {
             else if (a == "--max-inlier-rmse") policy.max_inlier_rmse = std::atof(value("--max-inlier-rmse")), thresholds = true;
             else if (a == "--load-map") load_map_path = value("--load-map"), map_options = true;
             else if (a == "--save-map") save_map_path = value("--save-map"), map_options = true;
+            else if (a == "--freeze-prior") freeze_prior = true, map_options = true;
             else if (a == "--downsample-order") {
                 const std::string v = value("--downsample-order");
                 if (v != "0" && v != "1") throw std::runtime_error("--downsample-order takes 0 or 1");
@@ -280,6 +286,10 @@ int main(int argc, char **argv) {
     }
     if (thresholds && map_update != "gated") {
         std::fprintf(stderr, "kicp_replay: --min-inliers, --min-fitness and --max-inlier-rmse need --map-update gated\n");
+        return 2;
+    }
+    if (freeze_prior && load_map_path.empty()) {
+        std::fprintf(stderr, "kicp_replay: --freeze-prior freezes the map --load-map loads: it needs --load-map\n");
         return 2;
     }
     map_options = map_options || thresholds;
@@ -381,6 +391,7 @@ int main(int argc, char **argv) {
         std::vector<uint64_t> digests;
         std::vector<kicp_corr_stats> corr;  // --correspondences: every frame's report, in frame order (last repetition)
         int64_t map_points = 0;  // the local map's size after the last frame
+        int64_t map_voxels = 0, prior_voxels = 0, prior_points = 0;  // --freeze-prior: the layers after the last repetition
         int64_t live_written = 0, live_records = 0;  // --publish live, last repetition: records written, and published, over all frames
         double map_seconds = 0.0;  // --publish, last repetition: time spent publishing the local map
         int64_t outcomes[KICP_FRAME_UPDATE_NONE + 1] = {};  // frames of the last repetition per KICP_FRAME_UPDATE_* outcome
@@ -392,6 +403,7 @@ int main(int argc, char **argv) {
                 kicp::check(kicp_map_load_voxels(pipeline.VoxelMap().handle_, prior.keys.data(), prior.counts.data(), prior.points.data(),
                                                  prior.num_voxels()),
                             "kicp_map_load_voxels");
+            if (freeze_prior) kicp::check(kicp_map_freeze(pipeline.VoxelMap().handle_), "kicp_map_freeze");
             for (int64_t &o : outcomes) o = 0;
             poses.clear();
             poses.reserve((size_t)n_frames);
@@ -498,6 +510,10 @@ int main(int argc, char **argv) {
             seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
             rep_seconds.push_back(seconds);
             kicp::check(kicp_map_num_points(pipeline.VoxelMap().handle_, &map_points), "kicp_map_num_points");
+            if (freeze_prior) {
+                kicp::check(kicp_map_prior_size(pipeline.VoxelMap().handle_, &prior_voxels, &prior_points), "kicp_map_prior_size");
+                kicp::check(kicp_map_num_voxels(pipeline.VoxelMap().handle_, &map_voxels), "kicp_map_num_voxels");
+            }
             if (!save_map_path.empty() && rep == repeat - 1) {  // the map after the last repetition, as kicp_map_export_voxels gives it
                 kicp_map *h = pipeline.VoxelMap().handle_;
                 kicp::MapFile out;
@@ -558,6 +574,12 @@ int main(int argc, char **argv) {
                           (long long)outcomes[KICP_FRAME_UPDATE_REJECTED], (long long)outcomes[KICP_FRAME_UPDATE_SKIPPED],
                           (long long)outcomes[KICP_FRAME_UPDATE_NONE]);
             live += buf;
+            if (freeze_prior) {
+                std::snprintf(buf, sizeof(buf), ", \"prior_voxels\": %lld, \"prior_points\": %lld, \"live_voxels\": %lld, \"live_points\": %lld",
+                              (long long)prior_voxels, (long long)prior_points, (long long)(map_voxels - prior_voxels),
+                              (long long)(map_points - prior_points));
+                live += buf;
+            }
         }
         if (v3) {  // the slots, their kinds, and the odometry samples per frame (0: one motion per frame)
             live += ", \"slots\": " + std::to_string(drive.slots.size()) + ", \"slot_kinds\": [";

@@ -23,6 +23,7 @@
 //   blk[blocks_cap]    int4 {kx, ky, kz, count}  one header per occupied voxel ("block"), dense [0, num_blocks)
 //   pts[blocks_cap * cap * 4] double             block b owns points [b*cap, b*cap + count), insertion order;
 //                                                each point is {x, y, z, pad}: exactly one 32-byte sector
+//   blocks [0, prior_blocks) are a frozen prior when there is one (kicp_map_freeze): read-only, never evicted, never moved
 //
 // One 16-byte load resolves a probe to (block, count); a voxel's points are one contiguous <= cap*32 B run.
 // ---------------------------------------------------------------------------------------------------------
@@ -118,6 +119,13 @@ struct kicp_map {
     uint32_t *d_keep = nullptr, *d_new_id = nullptr;
     int4 *blk_spare = nullptr;
     double *pts_spare = nullptr;
+    // frozen prior (kicp_map_freeze): blocks [0, prior_blocks) never change and never move.  While frozen, blk_spare / pts_spare hold
+    // a copy of that prefix (so that the swap after a compaction keeps it), and prior_slots (its own allocation, prior_slots_cap
+    // slots) is the table as it holds the prior alone at the current nslots: an eviction restores it and re-inserts the live blocks.
+    uint32_t prior_blocks = 0;
+    int64_t prior_points = 0;
+    int4 *prior_slots = nullptr;
+    uint32_t prior_slots_cap = 0;
     // state of kicp_map_pointcloud_f32_live (kicp_map.cu), created by its first call
     struct MapLive *live = nullptr;
     // correspondence report (kicp_map.cu, created by its first use): the per-CTA partials of k_corr_eval for corr_grid CTAs, the

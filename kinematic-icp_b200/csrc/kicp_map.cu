@@ -285,19 +285,57 @@ static uint32_t next_pow2(uint64_t v) {
 // (Re)build the open-addressed table over the first `nslots` slots of the slab's table region (nslots <= slots_cap) from the first
 // `nb` blocks.  `ctr` (the frame path): the counters of the update just enqueued, from which k_table_rebuild reads the block count;
 // nb is then its upper bound.
-static int map_rebuild_table(kicp_map *m, uint32_t nslots, uint32_t nb, const uint32_t *ctr = nullptr) {
+// With a frozen prior of P blocks the table is the prior's snapshot plus blocks [P, nb): `restore` (after an eviction, same size and
+// slab) copies the snapshot in, in place of the clear; otherwise (a new size or a new slab) the prior is inserted first and the
+// snapshot taken from it.
+static int map_rebuild_table(kicp_map *m, uint32_t nslots, uint32_t nb, const uint32_t *ctr = nullptr, bool restore = false) {
     kicp_ctx *c = m->ctx;
     if (nslots > m->slots_cap) {
         kicp_set_error("voxel map: internal error, table larger than its slab region");
         return KICP_ERR_CAPACITY;
     }
     m->nslots = nslots;
-    KICP_CUDA(cudaMemsetAsync(m->slots, 0xFF, (size_t)m->nslots * sizeof(int4), c->stream));
-    if (nb) {
-        k_table_rebuild<<<(nb + 255) / 256, 256, 0, c->stream>>>(m->slots, m->nslots - 1, m->blk, nb, ctr);
+    const uint32_t P = m->prior_blocks;
+    const size_t table_bytes = (size_t)m->nslots * sizeof(int4);
+    if (P && restore) {
+        KICP_CUDA(cudaMemcpyAsync(m->slots, m->prior_slots, table_bytes, cudaMemcpyDeviceToDevice, c->stream));
+    } else {
+        KICP_CUDA(cudaMemsetAsync(m->slots, 0xFF, table_bytes, c->stream));
+        if (P) {
+            if (m->prior_slots_cap < m->nslots) {
+                KICP_CUDA(cudaStreamSynchronize(c->stream));
+                cudaFree(m->prior_slots);
+                m->prior_slots = nullptr, m->prior_slots_cap = 0;
+                KICP_CUDA(cudaMalloc(&m->prior_slots, (size_t)m->slots_cap * sizeof(int4)));
+                m->prior_slots_cap = m->slots_cap;
+            }
+            k_table_rebuild<<<(P + 255) / 256, 256, 0, c->stream>>>(m->slots, m->nslots - 1, m->blk, P);
+            KICP_CHECK_LAUNCH(c);
+            KICP_CUDA(cudaMemcpyAsync(m->prior_slots, m->slots, table_bytes, cudaMemcpyDeviceToDevice, c->stream));
+        }
+    }
+    if (nb > P) {
+        k_table_rebuild<<<(nb - P + 255) / 256, 256, 0, c->stream>>>(m->slots, m->nslots - 1, m->blk, nb, ctr, P);
         KICP_CHECK_LAUNCH(c);
     }
     return KICP_OK;
+}
+
+// the prior prefix [0, P) of the live arrays into the spare ones, which a compaction fills from block P on
+static int map_mirror_prior(kicp_map *m) {
+    const uint32_t P = m->prior_blocks;
+    if (!P) return KICP_OK;
+    kicp_ctx *c = m->ctx;
+    KICP_CUDA(cudaMemcpyAsync(m->blk_spare, m->blk, (size_t)P * sizeof(int4), cudaMemcpyDeviceToDevice, c->stream));
+    KICP_CUDA(cudaMemcpyAsync(m->pts_spare, m->pts, (size_t)P * m->cap * KICP_PSTRIDE * sizeof(double), cudaMemcpyDeviceToDevice,
+                              c->stream));
+    return KICP_OK;
+}
+
+static void map_prior_free(kicp_map *m) {
+    cudaFree(m->prior_slots);
+    m->prior_slots = nullptr, m->prior_slots_cap = 0;
+    m->prior_blocks = 0, m->prior_points = 0;
 }
 
 // All of a map's device storage is ONE allocation (the slab), carved into the arrays below for a capacity of `ncap` voxels.
@@ -336,6 +374,7 @@ static int map_alloc_storage(kicp_map *m, uint32_t ncap) {
     m->blk_spare = reinterpret_cast<int4 *>(slab + o_blk2), m->pts_spare = reinterpret_cast<double *>(slab + o_pts2);
     m->d_keep = reinterpret_cast<uint32_t *>(slab + o_keep), m->d_new_id = reinterpret_cast<uint32_t *>(slab + o_id);
     m->slots = reinterpret_cast<int4 *>(slab + o_slots), m->slots_cap = slots_cap;
+    KICP_TRY(map_mirror_prior(m));  // the new spare arrays hold the frozen prefix too
     // the table moved with the slab: rebuild it at its previous size (or the minimum for a new map)
     return map_rebuild_table(m, std::max<uint32_t>(std::min(m->nslots, slots_cap), 1024u), m->num_blocks);
 }
@@ -416,6 +455,7 @@ extern "C" int kicp_map_destroy(kicp_map *m) {
     cudaSetDevice(m->ctx->device);
     cudaStreamSynchronize(m->ctx->stream);
     cudaFree(m->slab), cudaFree(m->d_counters);
+    map_prior_free(m);
     cudaFree(m->d_in), cudaFree(m->d_xyz_t), cudaFree(m->d_next), cudaFree(m->d_touched), cudaFree(m->d_dist);
     cudaFree(m->d_corr_part), cudaFree(m->d_corr_stats), cudaFree(m->d_corr_inl);
     map_live_free(m);
@@ -431,6 +471,48 @@ extern "C" int kicp_map_clear(kicp_map *m) {
     m->num_blocks = 0, m->num_points = 0;
     KICP_CUDA(cudaMemsetAsync(m->slots, 0xFF, (size_t)m->nslots * sizeof(int4), m->ctx->stream));
     KICP_CUDA(cudaStreamSynchronize(m->ctx->stream));
+    map_prior_free(m);  // the prior goes with the content
+    return KICP_OK;
+}
+
+extern "C" int kicp_map_freeze(kicp_map *m) {
+    if (!m) return kicp_invalid("kicp_map_freeze", "null map");
+    kicp_ctx *c = m->ctx;
+    KICP_CUDA(cudaSetDevice(c->device));
+    if (m->num_blocks == 0) {  // nothing to freeze: no prior
+        KICP_CUDA(cudaStreamSynchronize(c->stream));
+        map_prior_free(m);
+        return KICP_OK;
+    }
+    // every voxel now in the table becomes prior, so the table as it stands is the prior's snapshot
+    if (m->prior_slots_cap < m->slots_cap) {
+        KICP_CUDA(cudaStreamSynchronize(c->stream));
+        cudaFree(m->prior_slots);
+        m->prior_slots = nullptr, m->prior_slots_cap = 0;
+        KICP_CUDA(cudaMalloc(&m->prior_slots, (size_t)m->slots_cap * sizeof(int4)));
+        m->prior_slots_cap = m->slots_cap;
+    }
+    KICP_CUDA(cudaMemcpyAsync(m->prior_slots, m->slots, (size_t)m->nslots * sizeof(int4), cudaMemcpyDeviceToDevice, c->stream));
+    m->prior_blocks = m->num_blocks, m->prior_points = m->num_points;
+    KICP_TRY(map_mirror_prior(m));
+    KICP_CUDA(cudaStreamSynchronize(c->stream));
+    return KICP_OK;
+}
+
+extern "C" int kicp_map_thaw(kicp_map *m) {
+    if (!m) return kicp_invalid("kicp_map_thaw", "null map");
+    KICP_CUDA(cudaSetDevice(m->ctx->device));
+    KICP_CUDA(cudaStreamSynchronize(m->ctx->stream));
+    map_prior_free(m);
+    return KICP_OK;
+}
+
+extern "C" int kicp_map_prior_size(kicp_map *m, int64_t *voxels, int64_t *points) {
+    static const char fn[] = "kicp_map_prior_size";
+    if (!voxels) return kicp_invalid(fn, "voxels: null pointer");
+    if (!points) return kicp_invalid(fn, "points: null pointer");
+    if (!m) return kicp_invalid(fn, "null map");
+    *voxels = m->prior_blocks, *points = m->prior_points;
     return KICP_OK;
 }
 extern "C" int kicp_map_empty(kicp_map *m, int32_t *empty) {
@@ -487,7 +569,7 @@ static int map_insert(kicp_map *m, const double *xyz, bool xyz_on_device, int64_
     if (pose7) pose = Pose{pose7[0], pose7[1], pose7[2], pose7[3], pose7[4], pose7[5], pose7[6]};
     const unsigned grid = (unsigned)((n + 255) / 256);
     k_add_find_or_create<<<grid, 256, 0, c->stream>>>(rw, xyz, n, pose7 || d_res ? 1 : 0, pose, m->d_xyz_t, m->d_next, m->d_counters,
-                                                     m->d_touched, d_n, d_res);
+                                                     m->d_touched, d_n, d_res, m->prior_blocks);
     KICP_CHECK_LAUNCH(c);
     // KISS AddPoints: map_resolution = sqrt(voxel_size^2 / max_points_per_voxel)
     const double map_resolution = std::sqrt(m->voxel_size * m->voxel_size / (double)m->cap);
@@ -502,12 +584,18 @@ static int map_insert(kicp_map *m, const double *xyz, bool xyz_on_device, int64_
 // status are read from `d_res` on the device (`origin` is unused) and the block count from the insert's counters (nb is its upper
 // bound).  Nothing is read back and the compaction always runs — a moving sensor evicts voxels on practically every frame anyway,
 // and the host cannot know.
+// With a frozen prior of P blocks every step runs over the suffix [P, nb) only: the prior never dies, the spare arrays already hold
+// its copy at [0, P), and the table is restored from the prior's snapshot before the live blocks are re-inserted.  Each step is still
+// one launch.
 static int map_evict(kicp_map *m, const double origin[3], const kicp_reg_result *d_res, uint32_t nb) {
     kicp_ctx *c = m->ctx;
+    const uint32_t P = m->prior_blocks;
+    if (nb <= P) return KICP_OK;  // (synchronous only: the frame path's bound exceeds the block count) nothing can die
+    const uint32_t nl = nb - P;
     const uint32_t init[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     if (!d_res) KICP_CUDA(cudaMemcpyAsync(m->d_counters, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
-    k_mark_far<<<(nb + 255) / 256, 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, nb, origin[0], origin[1], origin[2],
-                                                       m->max_distance * m->max_distance, m->d_keep, m->d_counters, d_res);
+    k_mark_far<<<(nl + 255) / 256, 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, nb, origin[0], origin[1], origin[2],
+                                                       m->max_distance * m->max_distance, m->d_keep, m->d_counters, d_res, P);
     KICP_CHECK_LAUNCH(c);
     uint32_t res[8];
     if (!d_res) {
@@ -515,14 +603,15 @@ static int map_evict(kicp_map *m, const double origin[3], const kicp_reg_result 
         KICP_CUDA(cudaStreamSynchronize(c->stream));
         if (res[4] == 0) return KICP_OK;
     }
-    KICP_TRY(enqueue_exclusive_sum(c, m->d_keep, m->d_new_id, nb));
-    k_compact_blocks<<<(unsigned)(((uint64_t)nb * 32 + 255) / 256), 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, nb, m->d_keep,
-                                                                                       m->d_new_id, m->blk_spare, m->pts_spare);
+    KICP_TRY(enqueue_exclusive_sum(c, m->d_keep + P, m->d_new_id + P, nl));
+    k_compact_blocks<<<(unsigned)(((uint64_t)nl * 32 + 255) / 256), 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, nb, m->d_keep,
+                                                                                       m->d_new_id, m->blk_spare, m->pts_spare, P);
     KICP_CHECK_LAUNCH(c);
     std::swap(m->blk, m->blk_spare);
     std::swap(m->pts, m->pts_spare);
     if (!d_res) KICP_TRY(kicp_map_finish_update(m, res, true));
-    return map_rebuild_table(m, m->nslots, d_res ? nb : m->num_blocks, d_res ? m->d_counters : nullptr);  // after the compaction
+    // after the compaction
+    return map_rebuild_table(m, m->nslots, d_res ? nb : m->num_blocks, d_res ? m->d_counters : nullptr, true);
 }
 
 // AddPoints with the count and the pose on the host: one synchronisation, after which the host mirrors are current
@@ -624,46 +713,72 @@ int kicp_map_update_pose_async(kicp_map *m, const double *d_xyz, int64_t n_max, 
 // Pointcloud / export: the stored points are packed ON THE DEVICE (k_block_counts + k_exclusive_sum + k_pack_points, block order,
 // insertion order inside a block — the order the host loop used to produce) and exactly num_points * sizeof(T) * 3 bytes cross PCIe,
 // instead of the padded block array (20 slots of 32 bytes per voxel whatever it holds).  The spare point array is the scratch: it
-// holds nothing between two evictions.
-// packed xyz of every stored point -> host `out_xyz` (num_points * 3 doubles, or float32 records for T = float); headers -> `hdr`
+// holds nothing between two evictions but the mirrored prior prefix [0, P), so the packing starts after it (or, when the rest of the
+// spare is too small for the packed cloud, goes to a buffer of this call).
+// One layer (KICP_MAP_LAYER_*) is one range of blocks: ALL [0, nb), PRIOR [0, P), LIVE [P, nb).
+struct LayerRange {
+    uint32_t b0, nb;
+    int64_t points;
+};
+static LayerRange map_layer(const kicp_map *m, int layer) {
+    const uint32_t P = m->prior_blocks;
+    if (layer == KICP_MAP_LAYER_PRIOR) return LayerRange{0, P, m->prior_points};
+    if (layer == KICP_MAP_LAYER_LIVE) return LayerRange{P, m->num_blocks - P, m->num_points - m->prior_points};
+    return LayerRange{0, m->num_blocks, m->num_points};
+}
+// packed xyz of the layer's stored points -> host `out_xyz` (points * 3 doubles, or float32 records for T = float); headers -> `hdr`
 // when asked for.  A `device` out_xyz is packed into directly, on the context stream, without a copy or a host synchronisation.
 template <class T>
-static int map_download_packed(kicp_map *m, T *out_xyz, std::vector<int4> *hdr, bool device = false) {
+static int map_download_packed(kicp_map *m, T *out_xyz, std::vector<int4> *hdr, bool device = false, int layer = KICP_MAP_LAYER_ALL) {
     kicp_ctx *c = m->ctx;
     KICP_CUDA(cudaSetDevice(c->device));
-    if (m->num_blocks == 0) return KICP_OK;
-    k_block_counts<<<(m->num_blocks + 255) / 256, 256, 0, c->stream>>>(m->blk, m->num_blocks, m->d_keep);
+    const LayerRange L = map_layer(m, layer);
+    if (L.nb == 0) return KICP_OK;
+    const int4 *blk = m->blk + L.b0;
+    const double *pts = m->pts + (size_t)L.b0 * m->cap * KICP_PSTRIDE;
+    k_block_counts<<<(L.nb + 255) / 256, 256, 0, c->stream>>>(blk, L.nb, m->d_keep);
     KICP_CHECK_LAUNCH(c);
-    if (m->num_points >= (1ll << 30)) {
+    if (L.points >= (1ll << 30)) {
         kicp_set_error("voxel map: export of 2^30 points or more is not supported");
         return KICP_ERR_CAPACITY;
     }
-    KICP_TRY(enqueue_exclusive_sum(c, m->d_keep, m->d_new_id, m->num_blocks));
-    T *packed = device ? out_xyz : reinterpret_cast<T *>(m->pts_spare);
-    k_pack_points<T><<<(unsigned)(((uint64_t)m->num_blocks * 32 + 255) / 256), 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, m->num_blocks,
-                                                                                                   m->d_new_id, packed);
-    KICP_CHECK_LAUNCH(c);
-    if (device) return KICP_OK;
-    KICP_CUDA(cudaMemcpyAsync(out_xyz, packed, (size_t)m->num_points * 3 * sizeof(T), cudaMemcpyDeviceToHost, c->stream));
-    if (hdr) {
-        hdr->resize(m->num_blocks);
-        KICP_CUDA(cudaMemcpyAsync(hdr->data(), m->blk, hdr->size() * sizeof(int4), cudaMemcpyDeviceToHost, c->stream));
+    KICP_TRY(enqueue_exclusive_sum(c, m->d_keep, m->d_new_id, L.nb));
+    const size_t spare_off = (size_t)m->prior_blocks * m->cap * KICP_PSTRIDE;
+    const size_t spare_room = ((size_t)m->blocks_cap * m->cap * KICP_PSTRIDE - spare_off) * sizeof(double);
+    const size_t packed_bytes = (size_t)L.points * 3 * sizeof(T);
+    T *scratch = nullptr;
+    if (!device && packed_bytes > spare_room) KICP_CUDA(cudaMalloc(&scratch, packed_bytes));
+    T *packed = device ? out_xyz : scratch ? scratch : reinterpret_cast<T *>(m->pts_spare + spare_off);
+    k_pack_points<T><<<(unsigned)(((uint64_t)L.nb * 32 + 255) / 256), 256, 0, c->stream>>>(blk, pts, (int)m->cap, L.nb, m->d_new_id,
+                                                                                          packed);
+    c->launches++;  // KICP_CHECK_LAUNCH, with the scratch freed on every path
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess && !device) {
+        e = cudaMemcpyAsync(out_xyz, packed, packed_bytes, cudaMemcpyDeviceToHost, c->stream);
+        if (e == cudaSuccess && hdr) {
+            hdr->resize(L.nb);
+            e = cudaMemcpyAsync(hdr->data(), blk, hdr->size() * sizeof(int4), cudaMemcpyDeviceToHost, c->stream);
+        }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     }
-    KICP_CUDA(cudaStreamSynchronize(c->stream));
+    cudaFree(scratch);
+    if (e != cudaSuccess) return kicp_cuda_fail(e, "map_download_packed", __FILE__, __LINE__);
     return KICP_OK;
 }
 
 template <class T>
-static int map_pointcloud(kicp_map *m, T *out_xyz, int64_t cap, int64_t *n, bool device = false) {
+static int map_pointcloud(kicp_map *m, T *out_xyz, int64_t cap, int64_t *n, bool device = false, int layer = KICP_MAP_LAYER_ALL,
+                          const char *fn = "kicp_map_pointcloud_device_async") {
     if (!m || !n || (device && !out_xyz)) return KICP_ERR_INVALID;
-    *n = m->num_points;
+    const int64_t points = map_layer(m, layer).points;
+    *n = points;
     if (device)
-        KICP_TRY(kicp_check_device_range(m->ctx, out_xyz, (size_t)std::max<int64_t>(1, std::min(cap, m->num_points)) * 3 * sizeof(T),
-                                         sizeof(T), "kicp_map_pointcloud_device_async: out"));
-    if (m->num_points > cap) return KICP_ERR_CAPACITY;
-    if (m->num_points == 0) return KICP_OK;
+        KICP_TRY(kicp_check_device_range(m->ctx, out_xyz, (size_t)std::max<int64_t>(1, std::min(cap, points)) * 3 * sizeof(T),
+                                         sizeof(T), (std::string(fn) + ": out").c_str()));
+    if (points > cap) return KICP_ERR_CAPACITY;
+    if (points == 0) return KICP_OK;
     if (!out_xyz) return KICP_ERR_INVALID;
-    return map_download_packed(m, out_xyz, nullptr, device);
+    return map_download_packed(m, out_xyz, nullptr, device, layer);
 }
 
 extern "C" int kicp_map_pointcloud(kicp_map *m, double *out_xyz, int64_t cap, int64_t *n) { return map_pointcloud(m, out_xyz, cap, n); }
@@ -677,6 +792,26 @@ extern "C" int kicp_map_pointcloud_device_async(kicp_map *m, void *out, int32_t 
     if (dtype == KICP_DTYPE_F64) return map_pointcloud(m, static_cast<double *>(out), cap, n, true);
     if (dtype == KICP_DTYPE_F32) return map_pointcloud(m, static_cast<float *>(out), cap, n, true);
     return KICP_ERR_INVALID;
+}
+
+// one layer of the map (KICP_MAP_LAYER_*), by the rules of the whole-map calls above; the arguments are checked before the map
+static int map_pointcloud_layer(kicp_map *m, int32_t layer, int32_t dtype, void *out, int64_t cap, int64_t *n, bool device, const char *fn) {
+    if (layer != KICP_MAP_LAYER_ALL && layer != KICP_MAP_LAYER_PRIOR && layer != KICP_MAP_LAYER_LIVE)
+        return kicp_invalid(fn, "layer: not KICP_MAP_LAYER_ALL, KICP_MAP_LAYER_PRIOR or KICP_MAP_LAYER_LIVE");
+    if (dtype != KICP_DTYPE_F64 && dtype != KICP_DTYPE_F32) return kicp_invalid(fn, "dtype: not KICP_DTYPE_F64 or KICP_DTYPE_F32");
+    if (!n) return kicp_invalid(fn, "n: null pointer");
+    if (device && !out) return kicp_invalid(fn, "out: null pointer");
+    if (!m) return kicp_invalid(fn, "null map");
+    const int64_t points = map_layer(m, layer).points;
+    if (!device && !out && points > 0 && cap >= points) return kicp_invalid(fn, "out: null pointer");
+    if (dtype == KICP_DTYPE_F64) return map_pointcloud(m, static_cast<double *>(out), cap, n, device, layer, fn);
+    return map_pointcloud(m, static_cast<float *>(out), cap, n, device, layer, fn);
+}
+extern "C" int kicp_map_pointcloud_layer(kicp_map *m, int32_t layer, int32_t dtype, void *out, int64_t cap, int64_t *n) {
+    return map_pointcloud_layer(m, layer, dtype, out, cap, n, false, "kicp_map_pointcloud_layer");
+}
+extern "C" int kicp_map_pointcloud_layer_device_async(kicp_map *m, int32_t layer, int32_t dtype, void *out, int64_t cap, int64_t *n) {
+    return map_pointcloud_layer(m, layer, dtype, out, cap, n, true, "kicp_map_pointcloud_layer_device_async");
 }
 
 // ------------------------------------------------------------------------------------------- live local-map cloud

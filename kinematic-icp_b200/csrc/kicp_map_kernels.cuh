@@ -58,11 +58,14 @@ __device__ __forceinline__ void table_insert_unique(int4 *slots, uint32_t mask, 
     }
 }
 
-// `ctr` (optional): the block count lives on the device — blocks after the last AddPoints minus the ones just evicted
-__global__ void k_table_rebuild(int4 *slots, uint32_t mask_in, const int4 *blk, uint32_t num_blocks, const uint32_t *ctr = nullptr) {
+// `ctr` (optional): the block count lives on the device — blocks after the last AddPoints minus the ones just evicted.
+// `first`: only blocks [first, num_blocks) are inserted (a frozen prior prefix [0, first) is already in the table, restored from its
+// snapshot)
+__global__ void k_table_rebuild(int4 *slots, uint32_t mask_in, const int4 *blk, uint32_t num_blocks, const uint32_t *ctr = nullptr,
+                                uint32_t first = 0) {
     __shared__ uint32_t s_mask[32];
     const uint32_t mask = lane_private(mask_in, s_mask);  // divergence safety, see kicp_device.cuh
-    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t b = first + blockIdx.x * blockDim.x + threadIdx.x;
     if (ctr) num_blocks = min(num_blocks, ctr[0] - ctr[4]);
     if (b >= num_blocks) return;
     const int4 h = blk[b];
@@ -74,9 +77,11 @@ __global__ void k_table_rebuild(int4 *slots, uint32_t mask_in, const int4 *blk, 
 // Asynchronous frames (kicp_register_frame): the point count (`d_n`, n is then its upper bound) and the pose (`d_res`, the result
 // block of the registration that precedes this launch on the stream) are read from device memory; a registration that did not
 // end with KICP_OK (NaN pose) leaves the map untouched.
+// `prior_blocks`: blocks [0, prior_blocks) are a frozen prior (kicp_map_freeze); a point whose voxel is one of them is dropped.
 __global__ void k_add_find_or_create(MapRW m, const double *__restrict__ xyz, int64_t n, int has_pose, Pose pose,
                                      double *__restrict__ xyz_t, int32_t *__restrict__ pend_next, uint32_t *counters,
-                                     int32_t *__restrict__ touched, const int *d_n = nullptr, const kicp_reg_result *d_res = nullptr) {
+                                     int32_t *__restrict__ touched, const int *d_n = nullptr, const kicp_reg_result *d_res = nullptr,
+                                     uint32_t prior_blocks = 0) {
     __shared__ uint32_t s_mask[32];
     const uint32_t tmask = lane_private(m.mask, s_mask);  // divergence safety, see kicp_device.cuh
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -124,6 +129,7 @@ __global__ void k_add_find_or_create(MapRW m, const double *__restrict__ xyz, in
         }
         h = (h + 1) & tmask;
     }
+    if (block < prior_blocks) return;  // a frozen prior voxel: read-only
     const int32_t prev = atomicExch(&m.pend_head[block], (int32_t)i);
     pend_next[i] = prev;
     if (prev == -1) touched[atomicAdd(&counters[1], 1u)] = (int32_t)block;
@@ -214,9 +220,11 @@ __global__ void k_add_commit(MapRW m, const double *__restrict__ xyz_t, const in
 // `d_res` (asynchronous frames): the block count is counters[0] (num_blocks is its upper bound: the flags beyond it are
 // cleared for the scan that follows), the origin is the translation of the registration result, removed points are counted in
 // counters[5], and nothing dies after a registration that did not end with KICP_OK.
+// `first`: only blocks [first, num_blocks) are judged (and flagged); a frozen prior prefix [0, first) never dies.
 __global__ void k_mark_far(const int4 *blk, const double *pts, int cap, uint32_t num_blocks, double ox, double oy, double oz,
-                           double max_distance2, uint32_t *keep, uint32_t *counters, const kicp_reg_result *d_res = nullptr) {
-    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+                           double max_distance2, uint32_t *keep, uint32_t *counters, const kicp_reg_result *d_res = nullptr,
+                           uint32_t first = 0) {
+    const uint32_t b = first + blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= num_blocks) return;
     bool alive_only = false;
     if (d_res) {
@@ -237,13 +245,15 @@ __global__ void k_mark_far(const int4 *blk, const double *pts, int cap, uint32_t
     }
 }
 
+// `first`: only blocks [first, num_blocks) move; new_id[b] counts the survivors in [first, b), so block b lands at first + new_id[b]
+// (the prefix [0, first) is a frozen prior, which the spare arrays already hold)
 __global__ void k_compact_blocks(const int4 *blk, const double *pts, int cap, uint32_t num_blocks, const uint32_t *keep,
-                                 const uint32_t *new_id, int4 *blk_out, double *pts_out) {
+                                 const uint32_t *new_id, int4 *blk_out, double *pts_out, uint32_t first = 0) {
     // one warp per block: header by lane 0, points copied cooperatively (blocks beyond the live count carry keep = 0)
-    const uint32_t b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t b = first + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     const int lane = threadIdx.x & 31;
     if (b >= num_blocks || !keep[b]) return;
-    const uint32_t nb = new_id[b];
+    const uint32_t nb = first + new_id[b];
     const int4 h = blk[b];
     if (lane == 0) blk_out[nb] = h;
     const double *src = pts + (size_t)b * cap * KICP_PSTRIDE;

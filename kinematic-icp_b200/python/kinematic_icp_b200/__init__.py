@@ -211,6 +211,20 @@ def pinned_result():
     return RegResult.from_address(p.value)
 
 
+_LAYERS = {"all": _capi.KICP_MAP_LAYER_ALL, "prior": _capi.KICP_MAP_LAYER_PRIOR, "live": _capi.KICP_MAP_LAYER_LIVE}
+
+
+def _layer_code(layer):
+    """None (the whole map through the calls without a layer), a KICP_MAP_LAYER_* code, or its name"""
+    if layer is None:
+        return None
+    if isinstance(layer, str):
+        if layer not in _LAYERS:
+            raise ValueError("layer: one of %s" % ", ".join(sorted(_LAYERS)))
+        return _LAYERS[layer]
+    return int(layer)
+
+
 class VoxelHashMap:
     """kiss_icp::VoxelHashMap(voxel_size, max_distance, max_points_per_voxel), resident in HBM."""
 
@@ -290,30 +304,72 @@ class VoxelHashMap:
         else:
             check(lib().kicp_map_update_pose(self.h, dp(points), len(points), dp(a)), "kicp_map_update_pose")
 
-    def Pointcloud(self):
-        n = self.num_points()
-        out = np.empty((max(n, 1), 3))
+    def freeze(self):
+        """kicp_map_freeze: every voxel now in the map becomes a read-only prior that Update never evicts and AddPoints never writes
+        into; the voxels added later form the live layer beside it.  A second freeze also takes in the live voxels."""
+        check(lib().kicp_map_freeze(self.h), "kicp_map_freeze")
+
+    def thaw(self):
+        """kicp_map_thaw: the prior becomes ordinary voxels again (the next eviction may remove them)."""
+        check(lib().kicp_map_thaw(self.h), "kicp_map_thaw")
+
+    def _prior_size(self):
+        v, n = C.c_int64(), C.c_int64()
+        check(lib().kicp_map_prior_size(self.h, C.byref(v), C.byref(n)), "kicp_map_prior_size")
+        return v.value, n.value
+
+    def num_prior_voxels(self):
+        return self._prior_size()[0]
+
+    def num_prior_points(self):
+        return self._prior_size()[1]
+
+    def _layer_points(self, layer):
+        """the point count of a layer code (None: the whole map); 0 for a code the library refuses"""
+        if layer is None or layer == _capi.KICP_MAP_LAYER_ALL:
+            return self.num_points()
+        n = self._prior_size()[1]
+        return {_capi.KICP_MAP_LAYER_PRIOR: n, _capi.KICP_MAP_LAYER_LIVE: self.num_points() - n}.get(layer, 0)
+
+    def _pointcloud(self, layer, dtype):
+        n = self._layer_points(layer)
+        out = np.empty((max(n, 1), 3), dtype=dtype)
         m = C.c_int64()
-        check(lib().kicp_map_pointcloud(self.h, dp(out), n, C.byref(m)), "kicp_map_pointcloud")
+        if layer is None:
+            if dtype == np.float64:
+                check(lib().kicp_map_pointcloud(self.h, dp(out), n, C.byref(m)), "kicp_map_pointcloud")
+            else:
+                check(lib().kicp_map_pointcloud_f32(self.h, _capi.fp(out), n, C.byref(m)), "kicp_map_pointcloud_f32")
+        else:
+            code = _capi.KICP_DTYPE_F64 if dtype == np.float64 else _capi.KICP_DTYPE_F32
+            check(lib().kicp_map_pointcloud_layer(self.h, int(layer), code, out.ctypes.data, n, C.byref(m)), "kicp_map_pointcloud_layer")
         return out[: m.value].copy()
 
-    def PointcloudF32(self):
-        """Pointcloud() as the float32 (N, 3) records EigenToPointCloud2 publishes, narrowed on the device (kicp_map_pointcloud_f32)."""
-        n = self.num_points()
-        out = np.empty((max(n, 1), 3), dtype=np.float32)
-        m = C.c_int64()
-        check(lib().kicp_map_pointcloud_f32(self.h, _capi.fp(out), n, C.byref(m)), "kicp_map_pointcloud_f32")
-        return out[: m.value].copy()
+    def Pointcloud(self, layer=None):
+        """Pointcloud(); `layer` (KICP_MAP_LAYER_ALL / _PRIOR / _LIVE, or "all" / "prior" / "live"): one layer of a map with a frozen
+        prior (kicp_map_pointcloud_layer), ALL being PRIOR followed by LIVE."""
+        return self._pointcloud(_layer_code(layer), np.float64)
 
-    def PointcloudInto(self, out, stream=None):
+    def PointcloudF32(self, layer=None):
+        """Pointcloud() as the float32 (N, 3) records EigenToPointCloud2 publishes, narrowed on the device (kicp_map_pointcloud_f32);
+        `layer` as for Pointcloud."""
+        return self._pointcloud(_layer_code(layer), np.float32)
+
+    def PointcloudInto(self, out, stream=None, layer=None):
         """Pointcloud() (float64 `out`) or PointcloudF32()'s records (float32 `out`) written on the device into `out`, a contiguous
         (cap, 3) device array (__cuda_array_interface__), without a host synchronisation (kicp_map_pointcloud_device_async).  The
-        context waits for `stream` first and `stream` waits for the packing after; returns the point count n (rows [0, n) of `out`)."""
+        context waits for `stream` first and `stream` waits for the packing after; returns the point count n (rows [0, n) of `out`).
+        `layer` as for Pointcloud (kicp_map_pointcloud_layer_device_async)."""
         ptr, cap, code = _device.device_output(out, "PointcloudInto")
+        layer = _layer_code(layer)
         s = _device.resolve_stream(stream, out)
         self.ctx.wait_stream(s)
         n = C.c_int64()
-        check(lib().kicp_map_pointcloud_device_async(self.h, ptr, code, cap, C.byref(n)), "kicp_map_pointcloud_device_async")
+        if layer is None:
+            check(lib().kicp_map_pointcloud_device_async(self.h, ptr, code, cap, C.byref(n)), "kicp_map_pointcloud_device_async")
+        else:
+            check(lib().kicp_map_pointcloud_layer_device_async(self.h, layer, code, ptr, cap, C.byref(n)),
+                  "kicp_map_pointcloud_layer_device_async")
         self.ctx.stream_wait(s)
         return n.value
 

@@ -127,6 +127,7 @@ class MapLiveStats(C.Structure):
 
 
 KICP_DTYPE_F64, KICP_DTYPE_F32 = 0, 1
+KICP_MAP_LAYER_ALL, KICP_MAP_LAYER_PRIOR, KICP_MAP_LAYER_LIVE = 0, 1, 2  # kicp_map_pointcloud_layer
 KICP_STAGE_F64, KICP_STAGE_F32 = 1, 2  # kicp_frame_params.stage_clouds flags
 KICP_STAMP_NONE, KICP_STAMP_UINT32, KICP_STAMP_FLOAT32, KICP_STAMP_FLOAT64 = 0, 6, 7, 8  # PointField datatypes of a time field
 KICP_MAX_SENSORS, KICP_SENSOR_POINTS, KICP_SENSOR_LASER_SCAN = 8, 0, 1
@@ -178,6 +179,11 @@ SYMBOLS = [
     ("kicp_map_export_voxels", C.c_int, [_P, c_ip, c_ip, c_dp, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int64)]),
     ("kicp_map_load_voxels", C.c_int, [_P, c_ip, c_ip, c_dp, C.c_int64]),
+    ("kicp_map_freeze", C.c_int, [_P]),
+    ("kicp_map_thaw", C.c_int, [_P]),
+    ("kicp_map_prior_size", C.c_int, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    ("kicp_map_pointcloud_layer", C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
+    ("kicp_map_pointcloud_layer_device_async", C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
     ("kicp_map_nearest", C.c_int, [_P, c_dp, C.c_int64, c_dp, c_dp]),
     ("kicp_map_add_points_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     ("kicp_map_update_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp]),
