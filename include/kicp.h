@@ -224,6 +224,49 @@ int kicp_map_prior_size(kicp_map *map, int64_t *voxels, int64_t *points);
  * KICP_ERR_CAPACITY when cap < *n (nothing copied). */
 int kicp_map_pointcloud_layer(kicp_map *map, int32_t layer, int32_t dtype, void *out, int64_t cap, int64_t *n);
 int kicp_map_pointcloud_layer_device_async(kicp_map *map, int32_t layer, int32_t dtype, void *out, int64_t cap, int64_t *n);
+
+/* ---- free-space clearing: live voxels that a cloud's rays pass through leave the map (a van that drove off, a door that opened).
+ *      Inputs: the map (voxel size v, max_distance D, P prior voxels), n points p_i in a frame F, a pose T (F -> map) and a sensor
+ *      origin s in F, and the parameters below.  Plain IEEE double arithmetic with no contraction throughout:
+ *   1. o = T s and q_i = T p_i, the transform kicp_map_update_pose applies, bit for bit.
+ *   2. K(x) is the map's voxel key per axis (INT_MIN for a non-finite or huge value).  A ray is CAST when no coordinate of K(o) or
+ *      K(q_i) is INT_MIN; other rays do nothing.
+ *   3. Hit: a cast ray hits its end voxel K(q_i).
+ *   4. Misses: d = q_i - o, L = sqrt(dx*dx + dy*dy + dz*dz) (added in x, y, z order), t_end = min(L - end_margin, D) / L.  No voxel is
+ *      visited when L == 0 or t_end <= 0.  Otherwise a 3-D DDA runs from k = K(o).  Per axis j: d_j > 0: step +1,
+ *      tmax_j = ((k_j + 1) * v - o_j) / d_j, tdelta_j = v / d_j; d_j < 0: step -1, tmax_j = (k_j * v - o_j) / d_j, tdelta_j = -v / d_j;
+ *      d_j == 0: tmax_j = +inf (k_j + 1 and k_j * v in double).  Visit k; then at most |K(q_i) - K(o)|_1 times: take the axis j of the
+ *      smallest tmax (the lowest index on ties), stop if tmax_j >= t_end, else k_j += step_j, tmax_j += tdelta_j and visit k.  A visited
+ *      voxel that is in the map and is not K(q_i) gets one miss from this ray.
+ *   5. Decision: a LIVE voxel (block index >= P) with at least min_misses misses and no hit is cleared.  A prior voxel that meets the
+ *      condition is kept (prior voxels are read-only, kicp_map_freeze) and counted in prior_contradicted: its prior is going stale.
+ *   6. Removal: cleared voxels leave through the eviction's stable compaction; the survivors keep their relative order, so the exports
+ *      after the call are determined bit for bit.
+ *      The result depends only on integer counts: not on the order of the rays or on the launch shape.
+ *      Cost: one ray per point, one hash probe per voxel visited (up to about 3 D / v per ray); the map keeps one flag word per voxel
+ *      of capacity, allocated by its first clearing (a map that never clears allocates nothing). ------------------------------- */
+typedef struct kicp_free_space_params {
+    double end_margin;  /* metres cut from the end of every ray (>= 0, finite): keeps the voxels just before a hit */
+    int32_t min_misses; /* misses a live voxel needs to be cleared (>= 1; kicp_ctx_set_free_space: 0 = off) */
+} kicp_free_space_params;
+typedef struct kicp_free_space_stats {
+    int64_t rays;               /* rays cast */
+    int64_t visits;             /* voxels visited, summed over the cast rays */
+    int64_t cleared_voxels;     /* live voxels cleared */
+    int64_t cleared_points;     /* the points they held */
+    int64_t prior_contradicted; /* prior voxels that met the condition and were kept */
+} kicp_free_space_stats;
+/* The rule above for n host points at xyz.  Synchronous, with one host synchronisation; the host mirrors are current when it returns.
+ * `stats` may be NULL.  Errors: KICP_ERR_INVALID, with kicp_last_error naming the argument, for a null map, pose, sensor_origin or params,
+ * xyz == NULL with n > 0, n < 0 or n >= 2^40, a non-finite pose or origin, an end_margin that is NaN, negative or infinite, or
+ * min_misses < 1. */
+int kicp_map_clear_free_space(kicp_map *map, const double *xyz, int64_t n, const double pose[7], const double sensor_origin[3],
+                              const kicp_free_space_params *params, kicp_free_space_stats *stats);
+/* The same for n device points in kicp_map_nearest_device_async's layout and validation rules (packed float64 read in place, other
+ * layouts widened once into the map's buffer); synchronous like the host variant. */
+int kicp_map_clear_free_space_device(kicp_map *map, const void *data, int64_t n, int32_t dtype, int32_t point_step, int32_t offset_x,
+                                     int32_t offset_y, int32_t offset_z, const double pose[7], const double sensor_origin[3],
+                                     const kicp_free_space_params *params, kicp_free_space_stats *stats);
 /* GetClosestNeighbor(query) for n queries: (closest point, distance); (0,0,0), DBL_MAX when nothing is found. */
 int kicp_map_nearest(kicp_map *map, const double *queries, int64_t n, double *out_points, double *out_dist);
 /* ---- the map operators on clouds in device memory.  `data` holds n points of device memory of the context's device in the layout of
@@ -532,6 +575,21 @@ int kicp_ctx_set_map_update(kicp_ctx *ctx, const kicp_map_update_policy *policy)
  * returned KICP_OK or KICP_WARN_NO_CORRESPONDENCES, until the next front-end call.  Not a front-end call.  Errors: KICP_ERR_INVALID for
  * a null argument, named by kicp_last_error. */
 int kicp_frame_map_update(kicp_ctx *ctx, int32_t *outcome);
+/* Free-space clearing in the frame path (the rule of kicp_map_clear_free_space; default {0.0, 0}: off).  With min_misses >= 1 the
+ * single-sensor frame calls (kicp_register_frame, kicp_register_staged_frame, kicp_register_staged_frame_segments) clear the map after
+ * an Update whose outcome is KICP_FRAME_UPDATE_APPLIED: the points are frame_downsample (the cloud the Update inserts) in the base frame,
+ * the pose is the returned pose and the origin the translation of lidar_to_base.  The rays run against the map after the insert; a
+ * voxel the same Update evicts by distance counts as evicted, not cleared.  In the single-synchronisation order this is one memset and
+ * two more launches within the frame's one host synchronisation; the read-back order (option "frame_sync" 1, or small caller buffers)
+ * calls kicp_map_clear_free_space after its Update and gives the same map.  NEVER, a GATED rejection and a NaN pose leave the map
+ * untouched as before.  The multi-sensor calls (kicp_register_staged_sensors[_segments]) fail with KICP_ERR_INVALID while it is on (the
+ * down-sampled frame no longer knows which sensor a point came from): they consume the staged frame and leave the map unchanged; such a
+ * node calls kicp_map_clear_free_space once per sensor with that sensor's cloud.  Errors: KICP_ERR_INVALID, with kicp_last_error naming
+ * the field, for a null argument, an end_margin that is NaN, negative or infinite, or min_misses < 0; the previous setting is kept. */
+int kicp_ctx_set_free_space(kicp_ctx *ctx, const kicp_free_space_params *params);
+/* The statistics of the last frame call's clearing, with the correspondence report's lifetime: all zero when the option was off, the
+ * Update was not applied or the frame failed.  Not a front-end call.  Errors: KICP_ERR_INVALID for a null argument. */
+int kicp_frame_free_space(kicp_ctx *ctx, kicp_free_space_stats *stats);
 
 /* ---- the same frame in two steps, for a caller that needs the sweep's time range before it has the relative odometry (the
  *      online server: ProcessTimestamps -> wheel-odometry lookup over [begin, end] -> RegisterFrame,

@@ -255,6 +255,15 @@ int32_t KinematicICP::LastMapUpdate() const {
     kicp::check(kicp_frame_map_update(kicp::default_context(), &outcome), "kicp_frame_map_update");
     return outcome;
 }
+void KinematicICP::SetFreeSpace(int32_t min_misses, double end_margin) {
+    const kicp_free_space_params params{end_margin, min_misses};
+    kicp::check(kicp_ctx_set_free_space(kicp::default_context(), &params), "kicp_ctx_set_free_space");
+}
+kicp_free_space_stats KinematicICP::LastFreeSpace() const {
+    kicp_free_space_stats st{};
+    kicp::check(kicp_frame_free_space(kicp::default_context(), &st), "kicp_frame_free_space");
+    return st;
+}
 
 // the two clouds of the last frame, built in one pass each from the library's pinned staging
 KinematicICP::Vector3dVectorTuple KinematicICP::StagedClouds() {

@@ -151,6 +151,11 @@ public:
     // KICP_FRAME_UPDATE_* outcome of the last frame registered on it by any KinematicICP.  Both throw on an error the C call returns.
     static void SetMapUpdate(const kicp_map_update_policy &policy);
     int32_t LastMapUpdate() const;
+    // Extension: free-space clearing in the frame path of the process-wide context (kicp_ctx_set_free_space; min_misses 0 turns it
+    // off): after every applied Update the frame's down-sampled points clear the live voxels their rays pass through.  LastFreeSpace
+    // returns kicp_frame_free_space of that context.  Both throw on an error the C call returns.
+    static void SetFreeSpace(int32_t min_misses = 2, double end_margin = 0.5);
+    kicp_free_space_stats LastFreeSpace() const;
 
     void SetPose(const Sophus::SE3d &pose);  // also clears the map and the threshold statistics (KinematicICP.hpp:85-89)
 

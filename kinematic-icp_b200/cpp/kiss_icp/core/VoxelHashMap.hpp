@@ -67,6 +67,18 @@ struct VoxelHashMap {
         kicp::to_pose7(pose, p);
         kicp::check(kicp_map_update_pose(handle_, kicp::xyz(points), (int64_t)points.size(), p), "kicp_map_update_pose");
     }
+    // Free-space clearing (kicp_map_clear_free_space): every point of `points` (frame F) is a ray from pose * sensor_origin to
+    // pose * p; live voxels that at least min_misses rays pass through and in which no ray ends leave the map.  Throws on an error.
+    kicp_free_space_stats ClearFreeSpace(const std::vector<Eigen::Vector3d> &points, const Sophus::SE3d &pose,
+                                         const Eigen::Vector3d &sensor_origin, int32_t min_misses = 2, double end_margin = 0.5) {
+        double p[7];
+        kicp::to_pose7(pose, p);
+        const kicp_free_space_params params{end_margin, min_misses};
+        kicp_free_space_stats st{};
+        kicp::check(kicp_map_clear_free_space(handle_, kicp::xyz(points), (int64_t)points.size(), p, sensor_origin.data(), &params, &st),
+                    "kicp_map_clear_free_space");
+        return st;
+    }
     void AddPoints(const std::vector<Eigen::Vector3d> &points) {
         kicp::check(kicp_map_add_points(handle_, kicp::xyz(points), (int64_t)points.size()), "kicp_map_add_points");
     }

@@ -52,6 +52,11 @@
 // beside it.  "Localise on a prior map that keeps learning" is --load-map FILE --freeze-prior --map-update always (or gated).  The JSON
 // line then also reports the prior's and the live layer's voxel and point counts at the end of the last repetition ("prior_voxels",
 // "prior_points", "live_voxels", "live_points").
+// --free-space M[,E] switches on free-space clearing in the frame path of the default context (kicp.h kicp_ctx_set_free_space;
+// KinematicICP::SetFreeSpace) with min_misses M (>= 1) and end_margin E metres (default 0.5): after every applied Update the frame's
+// down-sampled points clear the live voxels their rays pass through.  The JSON line then reports "free_space" {min_misses,
+// end_margin} and the statistics summed over the last repetition's frames ("free_space_stats": rays, visits, cleared_voxels,
+// cleared_points, prior_contradicted).  A multi-sensor (KSEQ3 with several slots) drive is refused with it.
 //
 // Version 3, magic "KSEQ3\0\0\0", carries several message streams ("slots", 1..KICP_MAX_SENSORS: PointCloud2 records or 2D LaserScans,
 // each with its extrinsic) and the wheel odometry either as one relative motion or as poses sampled during the sweep:
@@ -230,7 +235,7 @@ int main(int argc, char **argv) {
         std::fprintf(stderr, "usage: %s drive.kseq out.tum [--deskew 0|1] [--voxel-size v] [--max-range r] [--min-range r] [--repeat k] [--pageable] "
                      "[--host-stamps] [--device-input] [--publish host|device|live] [--publish-digest FILE] [--downsample-order 0|1] "
                      "[--correspondences FILE] [--map-update always|never|gated] [--min-inliers k] [--min-fitness f] [--max-inlier-rmse r] "
-                     "[--load-map FILE] [--freeze-prior] [--save-map FILE]\n", argv[0]);
+                     "[--load-map FILE] [--freeze-prior] [--save-map FILE] [--free-space M[,E]]\n", argv[0]);
         return 2;
     }
     kinematic_icp::pipeline::Config config;  // the reference's defaults (pipeline/KinematicICP.hpp:38-60)
@@ -242,6 +247,7 @@ int main(int argc, char **argv) {
     std::string map_update = "always", load_map_path, save_map_path;
     kicp_map_update_policy policy{KICP_MAP_UPDATE_ALWAYS, 0, 0.0, HUGE_VAL};
     bool freeze_prior = false;  // --freeze-prior: freeze the map --load-map loaded
+    kicp_free_space_params free_space{0.5, 0};  // --free-space M[,E]; min_misses 0: off
     bool thresholds = false;  // a --min-* / --max-inlier-rmse option was given (only with --map-update gated)
     bool map_options = false;  // any of --map-update, the thresholds, --load-map, --save-map: the JSON line reports the outcomes
     for (int i = 3; i < argc; ++i) {
@@ -269,6 +275,21 @@ int main(int argc, char **argv) {
             else if (a == "--load-map") load_map_path = value("--load-map"), map_options = true;
             else if (a == "--save-map") save_map_path = value("--save-map"), map_options = true;
             else if (a == "--freeze-prior") freeze_prior = true, map_options = true;
+            else if (a == "--free-space") {
+                const std::string v = value("--free-space");
+                const size_t comma = v.find(',');
+                char *end = nullptr;
+                const long mm = std::strtol(v.c_str(), &end, 10);
+                if (end == v.c_str() || (comma == std::string::npos ? *end != '\0' : end != v.c_str() + comma) || mm < 1 || mm > INT32_MAX)
+                    throw std::runtime_error("--free-space takes M[,E]: min_misses M >= 1, end_margin E >= 0 metres");
+                free_space.min_misses = (int32_t)mm;
+                if (comma != std::string::npos) {
+                    const std::string e = v.substr(comma + 1);
+                    free_space.end_margin = std::strtod(e.c_str(), &end);
+                    if (e.empty() || *end != '\0' || !(free_space.end_margin >= 0.0) || std::isinf(free_space.end_margin))
+                        throw std::runtime_error("--free-space takes M[,E]: min_misses M >= 1, end_margin E >= 0 metres");
+                }
+            }
             else if (a == "--downsample-order") {
                 const std::string v = value("--downsample-order");
                 if (v != "0" && v != "1") throw std::runtime_error("--downsample-order takes 0 or 1");
@@ -318,6 +339,7 @@ int main(int argc, char **argv) {
             kicp::check(kicp_ctx_set_option(kicp::default_context(), "downsample_order", downsample_order), "--downsample-order");
         if (!corr_path.empty()) kinematic_icp::pipeline::KinematicICP::SetCorrespondences(true);
         if (map_options) kinematic_icp::pipeline::KinematicICP::SetMapUpdate(policy);  // a threshold out of range throws, naming the field
+        if (free_space.min_misses > 0) kinematic_icp::pipeline::KinematicICP::SetFreeSpace(free_space.min_misses, free_space.end_margin);
         kicp::MapFile prior;  // --load-map
         if (!load_map_path.empty()) {
             prior = kicp::read_map_file(load_map_path);
@@ -395,6 +417,7 @@ int main(int argc, char **argv) {
         int64_t live_written = 0, live_records = 0;  // --publish live, last repetition: records written, and published, over all frames
         double map_seconds = 0.0;  // --publish, last repetition: time spent publishing the local map
         int64_t outcomes[KICP_FRAME_UPDATE_NONE + 1] = {};  // frames of the last repetition per KICP_FRAME_UPDATE_* outcome
+        kicp_free_space_stats free_sum{};  // --free-space: the statistics summed over the last repetition's frames
         std::vector<double> rep_seconds;  // every repetition's wall time (a 24-frame drive lasts milliseconds: one hiccup halves a single figure)
         for (int rep = 0; rep < repeat; ++rep) {  // --repeat: the same drive again on a fresh pipeline (the last run is the one written)
             kinematic_icp::pipeline::KinematicICP pipeline(config);
@@ -405,6 +428,7 @@ int main(int argc, char **argv) {
                             "kicp_map_load_voxels");
             if (freeze_prior) kicp::check(kicp_map_freeze(pipeline.VoxelMap().handle_), "kicp_map_freeze");
             for (int64_t &o : outcomes) o = 0;
+            free_sum = kicp_free_space_stats{};
             poses.clear();
             poses.reserve((size_t)n_frames);
             digests.clear();
@@ -414,6 +438,11 @@ int main(int argc, char **argv) {
                 poses.emplace_back(stamp, pipeline.pose());
                 if (!corr_path.empty()) corr.push_back(pipeline.LastCorrespondenceStats());
                 ++outcomes[pipeline.LastMapUpdate()];
+                if (free_space.min_misses > 0) {
+                    const kicp_free_space_stats f = pipeline.LastFreeSpace();
+                    free_sum.rays += f.rays, free_sum.visits += f.visits, free_sum.cleared_voxels += f.cleared_voxels;
+                    free_sum.cleared_points += f.cleared_points, free_sum.prior_contradicted += f.prior_contradicted;
+                }
             };
             live_written = live_records = 0;
             map_seconds = 0.0;
@@ -580,6 +609,14 @@ int main(int argc, char **argv) {
                               (long long)(map_points - prior_points));
                 live += buf;
             }
+        }
+        if (free_space.min_misses > 0) {  // the free-space setting and its statistics over the last repetition's frames
+            char buf[384];
+            std::snprintf(buf, sizeof(buf), ", \"free_space\": {\"min_misses\": %d, \"end_margin\": %.17g}, \"free_space_stats\": {\"rays\": %lld, "
+                          "\"visits\": %lld, \"cleared_voxels\": %lld, \"cleared_points\": %lld, \"prior_contradicted\": %lld}",
+                          (int)free_space.min_misses, free_space.end_margin, (long long)free_sum.rays, (long long)free_sum.visits,
+                          (long long)free_sum.cleared_voxels, (long long)free_sum.cleared_points, (long long)free_sum.prior_contradicted);
+            live += buf;
         }
         if (v3) {  // the slots, their kinds, and the odometry samples per frame (0: one motion per frame)
             live += ", \"slots\": " + std::to_string(drive.slots.size()) + ", \"slot_kinds\": [";

@@ -166,6 +166,10 @@ struct Scratch {
     int32_t map_update = KICP_FRAME_UPDATE_NONE;
     kicp_reg_result *d_shadow = nullptr;
     int32_t *d_gate = nullptr, *h_gate = nullptr;
+    // free-space clearing (kicp_ctx_set_free_space): the last frame's statistics as kicp_frame_free_space returns them (the report's
+    // lifetime) and their pinned copy (allocated on the first frame with the option)
+    kicp_free_space_stats free_space = {};
+    kicp_free_space_stats *h_free = nullptr;
     double timing[8] = {0};  // host-side stage times of the last kicp_register_frame, milliseconds (debug export)
     int *first_idx = nullptr, *slot_of = nullptr, *d_count = nullptr;
     int4 *slots = nullptr;
@@ -188,7 +192,7 @@ void release(Scratch &s) {
     cudaFree(s.d_seg_mm), cudaFree(s.d_seg_count), cudaFreeHost(s.h_seg_mm), cudaFreeHost(s.h_seg_count);
     cudaFree(s.d_segs), cudaFreeHost(s.h_segs);
     cudaFree(s.corr_pts), cudaFree(s.corr_dist), cudaFree(s.corr_inl), cudaFreeHost(s.h_corr);
-    cudaFree(s.d_shadow), cudaFree(s.d_gate), cudaFreeHost(s.h_gate);
+    cudaFree(s.d_shadow), cudaFree(s.d_gate), cudaFreeHost(s.h_gate), cudaFreeHost(s.h_free);
     if (s.ev_segs) cudaEventDestroy(s.ev_segs);
     s.staged.release();
     if (s.ev_front) cudaEventDestroy(s.ev_front);
@@ -450,7 +454,7 @@ int open_frontend(kicp_ctx *c, int status, int64_t n) {
     if (c) {
         Scratch &s = scratch(c);
         s.held_n = -1, s.dev_n_frame = s.dev_n_source = 0;
-        s.corr_n = 0, s.corr = kicp_corr_stats{}, s.map_update = KICP_FRAME_UPDATE_NONE;
+        s.corr_n = 0, s.corr = kicp_corr_stats{}, s.map_update = KICP_FRAME_UPDATE_NONE, s.free_space = kicp_free_space_stats{};
     }
     if (status != KICP_OK) return status;
     KICP_CUDA(cudaSetDevice(c->device));
@@ -669,9 +673,15 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
     const bool never = policy.mode == KICP_MAP_UPDATE_NEVER, gated = policy.mode == KICP_MAP_UPDATE_GATED;
     const bool map_was_empty = map->num_points == 0;
     const bool corr = c->correspondences != 0 || gated;
-    s.corr_n = 0, s.corr = kicp_corr_stats{}, s.map_update = KICP_FRAME_UPDATE_NONE;
+    // free-space clearing after an applied Update: the frame's rays from the sensor origin in the base frame (lidar_to_base's translation)
+    const kicp_free_space_params fs = c->free_space;
+    const bool clear = fs.min_misses > 0 && !never;
+    const double fs_origin[3] = {a.lidar_to_base[4], a.lidar_to_base[5], a.lidar_to_base[6]};
+    kicp_free_space_stats free_st{};
+    s.corr_n = 0, s.corr = kicp_corr_stats{}, s.map_update = KICP_FRAME_UPDATE_NONE, s.free_space = kicp_free_space_stats{};
     // the report's buffers are sized before anything of this frame is enqueued: a growth (cudaFree / cudaMalloc) waits for the device
     if (corr) KICP_TRY(reserve_corr(s));
+    if (clear && !s.h_free) KICP_CUDA(cudaMallocHost(&s.h_free, sizeof(kicp_free_space_stats)));
     if (gated && one_sync) KICP_TRY(reserve_gate(s));
     // the survivor counts of the three stages (12 bytes back, one synchronisation of the stream)
     int counts[3] = {0, 0, 0};
@@ -743,7 +753,8 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
                 KICP_CUDA(cudaMemcpyAsync(s.h_gate, s.d_gate, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
                 d_res = s.d_shadow;
             }
-            KICP_TRY(kicp_map_update_pose_async(map, reinterpret_cast<const double *>(s.out2), n, s.d_count + 1, d_res, s.h_mapctr));
+            KICP_TRY(kicp_map_update_pose_async(map, reinterpret_cast<const double *>(s.out2), n, s.d_count + 1, d_res, s.h_mapctr,
+                                                clear ? &fs : nullptr, fs_origin, s.h_free));
         }
         KICP_TRY(read_counts());  // THE synchronisation of the frame
     } else {
@@ -761,8 +772,12 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
     if (one_sync) {
         const int mst = never ? KICP_OK : kicp_map_finish_update(map, s.h_mapctr, false);
         if (mst != KICP_OK) status = mst;
+        if (clear) free_st = *s.h_free;
     } else if (outcome == KICP_FRAME_UPDATE_APPLIED && counts[1] > 0) {
         status = kicp_map_update_pose_packed(map, reinterpret_cast<const double *>(s.out2), counts[1], r.pose);
+        if (status == KICP_OK && clear)
+            status = kicp_map_clear_free_space_packed(map, reinterpret_cast<const double *>(s.out2), counts[1], r.pose, fs_origin, &fs,
+                                                      &free_st);
     }
     s.timing[3] = ms_since();  // + map update
     if (counts[2] > src_copy) KICP_TRY(s.staged.fetch(c->copy_stream, s.out, s.out3, stage, stage32, 0, src_copy, counts[2]));
@@ -772,6 +787,7 @@ int register_ingested(kicp_map *map, Scratch &s, const FrameArgs &a) {
         s.dev_n_frame = counts[0], s.dev_n_source = counts[2], s.dev_f32 = stage32;
         if (corr) s.corr_n = counts[2], s.corr = *s.h_corr;
         s.map_update = outcome;
+        s.free_space = free_st;
     }
     s.timing[4] = ms_since();  // + clouds delivered
     return status;
@@ -1102,6 +1118,10 @@ extern "C" int kicp_frame_stage_sensors(kicp_ctx *c, const kicp_sensor_input *se
     return KICP_OK;
 }
 
+// The multi-sensor frame calls refuse free-space clearing: the down-sampled frame no longer knows which sensor a point came from
+static const char kMultiSensorFree[] =
+    "free-space clearing (kicp_ctx_set_free_space) needs a single-sensor frame: clear once per sensor with kicp_map_clear_free_space";
+
 // The second half for K sensors: kicp_register_staged_frame with a de-skew motion and an extrinsic per sensor of the staged frame.
 extern "C" int kicp_register_staged_sensors(kicp_map *map, int32_t k, const double deskew_motions[][7], const double lidar_to_bases[][7],
                                             const double last_pose[7], const double relative_odometry[7], double tau,
@@ -1116,7 +1136,9 @@ extern "C" int kicp_register_staged_sensors(kicp_map *map, int32_t k, const doub
                 std::chrono::steady_clock::now()};
     a.deskew_motions = deskew_motions, a.lidar_to_bases = lidar_to_bases;
     // the staged frame is consumed, whatever the outcome (its points are in the scratch already)
-    KICP_TRY(open_frontend(map->ctx, a.n >= 0 && k == s.held_k && a.valid() ? KICP_OK : KICP_ERR_INVALID, a.n));
+    int valid = a.n >= 0 && k == s.held_k && a.valid() ? KICP_OK : KICP_ERR_INVALID;
+    if (valid == KICP_OK && map->ctx->free_space.min_misses > 0) valid = kicp_invalid("kicp_register_staged_sensors", kMultiSensorFree);
+    KICP_TRY(open_frontend(map->ctx, valid, a.n));
     if (n_frame) *n_frame = 0;
     if (n_source) *n_source = 0;
     return register_ingested(map, s, a);
@@ -1184,6 +1206,7 @@ int register_staged_segments(kicp_map *map, int32_t k, const int32_t *n_segments
         if (s.held_n < 0) return kicp_invalid(fn, "no staged frame");
         if (single && s.held_k != 1) return kicp_invalid(fn, "the staged frame has several sensors");
         if (k != s.held_k) return kicp_invalid(fn, "k differs from the staged frame's sensor count");
+        if (!single && c->free_space.min_misses > 0) return kicp_invalid(fn, kMultiSensorFree);
         for (int i = 0; i < k; ++i) {
             const std::string where = single ? "segments" : "segments[" + std::to_string(i) + "]";
             KICP_TRY(check_segments(fn, where, n_segments[i], segments[i], deskew && s.held[i].stamped, s.held_range));
@@ -1330,6 +1353,25 @@ extern "C" int kicp_ctx_set_map_update(kicp_ctx *c, const kicp_map_update_policy
     if (!(p.max_inlier_rmse > 0.0)) return kicp_invalid(fn, "policy->max_inlier_rmse: not > 0");
     if (!c) return kicp_invalid(fn, "null context");
     c->map_update = p;
+    return KICP_OK;
+}
+
+// The free-space clearing of the frame calls: checked field by field, the context last; a failing call keeps the previous setting
+extern "C" int kicp_ctx_set_free_space(kicp_ctx *c, const kicp_free_space_params *params) {
+    static const char fn[] = "kicp_ctx_set_free_space";
+    if (!params) return kicp_invalid(fn, "params: null pointer");
+    KICP_TRY(kicp_check_free_space_params(fn, params, true));
+    if (!c) return kicp_invalid(fn, "null context");
+    c->free_space = *params;
+    return KICP_OK;
+}
+
+// The free-space statistics of the last frame call; not a front-end call
+extern "C" int kicp_frame_free_space(kicp_ctx *c, kicp_free_space_stats *stats) {
+    static const char fn[] = "kicp_frame_free_space";
+    if (!stats) return kicp_invalid(fn, "stats: null pointer");
+    if (!c) return kicp_invalid(fn, "null context");
+    *stats = scratch(c).free_space;
     return KICP_OK;
 }
 

@@ -70,6 +70,8 @@ struct kicp_ctx {
     int correspondences = 0;   // option "correspondences": 1 = the frame calls evaluate the source at the returned pose (kicp_frontend.cu)
     // kicp_ctx_set_map_update: whether the frame calls end with the map's Update (kicp_frontend.cu)
     kicp_map_update_policy map_update = {KICP_MAP_UPDATE_ALWAYS, 0, 0.0, INFINITY};
+    // kicp_ctx_set_free_space: whether the single-sensor frame calls clear free space after their Update (min_misses 0: off)
+    kicp_free_space_params free_space = {0.0, 0};
     int overlap_upload = 1;
     // the registration's device state, neighbour cache, upload flags and profiling records (kicp_register_api.cu owns the type)
     struct RegScratch *reg = nullptr;
@@ -126,6 +128,11 @@ struct kicp_map {
     int64_t prior_points = 0;
     int4 *prior_slots = nullptr;
     uint32_t prior_slots_cap = 0;
+    // free-space clearing (kicp_map.cu, allocated by the first clearing): the statistics words and, after them, one flag word per block
+    // for free_cap blocks (grown with blocks_cap)
+    unsigned long long *d_free_stats = nullptr;
+    uint32_t *d_free_flags = nullptr;
+    uint32_t free_cap = 0;
     // state of kicp_map_pointcloud_f32_live (kicp_map.cu), created by its first call
     struct MapLive *live = nullptr;
     // correspondence report (kicp_map.cu, created by its first use): the per-CTA partials of k_corr_eval for corr_grid CTAs, the
@@ -201,9 +208,17 @@ int kicp_check_cloud_args(const kicp_frame_input *in, const char *fn);
 int kicp_check_device_cloud(kicp_ctx *c, const kicp_frame_input *in, const char *fn, bool *packed);
 // defined in kicp_frontend.cu: k_ingest of such a checked cloud of n > 0 points into packed doubles at dst, on the context stream
 int kicp_enqueue_widen(kicp_ctx *c, const kicp_frame_input *in, double *dst);
-// the same with the point count and the pose still on the device (no read-back; kicp_map.cu)
+// the same with the point count and the pose still on the device (no read-back; kicp_map.cu).  `fs` (optional): free-space clearing of
+// the frame's rays from `fs_origin` (in the cloud's frame) after the insert, its statistics copied to `h_fs` (pinned) on the stream
 int kicp_map_update_pose_async(kicp_map *m, const double *d_xyz, int64_t n_max, const int *d_n, const kicp_reg_result *d_res,
-                               uint32_t *h_counters);
+                               uint32_t *h_counters, const kicp_free_space_params *fs = nullptr, const double fs_origin[3] = nullptr,
+                               kicp_free_space_stats *h_fs = nullptr);
+// kicp_map_clear_free_space with `d_xyz` already resident in HBM (packed xyz doubles) and checked arguments: used by the read-back
+// order of the frame calls
+int kicp_map_clear_free_space_packed(kicp_map *m, const double *d_xyz, int64_t n, const double pose[7], const double origin[3],
+                                     const kicp_free_space_params *p, kicp_free_space_stats *stats);
+// the checks of kicp_free_space_params (`allow_off`: min_misses 0, the frame path's "off", passes), KICP_ERR_INVALID naming the field
+int kicp_check_free_space_params(const char *fn, const kicp_free_space_params *p, bool allow_off);
 // the host mirrors from the counters an update copied back (`evict_only`: those of RemovePointsFarFromLocation alone)
 int kicp_map_finish_update(kicp_map *m, const uint32_t *ctr, bool evict_only);
 // device address of the result block the last enqueued registration on this context writes (kicp_register_api.cu)

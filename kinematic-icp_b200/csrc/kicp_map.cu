@@ -454,7 +454,7 @@ extern "C" int kicp_map_destroy(kicp_map *m) {
     if (!m) return KICP_OK;
     cudaSetDevice(m->ctx->device);
     cudaStreamSynchronize(m->ctx->stream);
-    cudaFree(m->slab), cudaFree(m->d_counters);
+    cudaFree(m->slab), cudaFree(m->d_counters), cudaFree(m->d_free_stats);
     map_prior_free(m);
     cudaFree(m->d_in), cudaFree(m->d_xyz_t), cudaFree(m->d_next), cudaFree(m->d_touched), cudaFree(m->d_dist);
     cudaFree(m->d_corr_part), cudaFree(m->d_corr_stats), cudaFree(m->d_corr_inl);
@@ -578,6 +578,49 @@ static int map_insert(kicp_map *m, const double *xyz, bool xyz_on_device, int64_
     return KICP_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------- free-space clearing
+#include "kicp_free_space_kernels.cuh"  // FreeRayArgs, k_free_rays, k_mark_free
+
+// The map's free-space words, one allocation beside the slab: kFreeStatWords statistics words, then one flag word per block of
+// capacity.  Allocated on the first clearing and grown with the block capacity (the stream drained first); a map that never clears
+// has none.
+static int free_reserve(kicp_map *m) {
+    if (m->free_cap >= m->blocks_cap) return KICP_OK;
+    KICP_CUDA(cudaStreamSynchronize(m->ctx->stream));
+    cudaFree(m->d_free_stats);
+    m->d_free_stats = nullptr, m->d_free_flags = nullptr, m->free_cap = 0;
+    void *p = nullptr;
+    KICP_CUDA(cudaMalloc(&p, kFreeStatWords * sizeof(unsigned long long) + (size_t)m->blocks_cap * sizeof(uint32_t)));
+    m->d_free_stats = static_cast<unsigned long long *>(p);
+    m->d_free_flags = reinterpret_cast<uint32_t *>(m->d_free_stats + kFreeStatWords);
+    m->free_cap = m->blocks_cap;
+    return KICP_OK;
+}
+
+// One memset (the statistics and the flags of blocks [0, nb)), then k_free_rays over the n rays of d_xyz (packed doubles) at `pose7`
+// (host) or at the pose of `d_res` with the count min(*d_n, n); the grid is at most the resident one (the warps stride over the rest)
+static int enqueue_free_rays(kicp_map *m, const double *d_xyz, int64_t n, const int *d_n, const double *pose7, const kicp_reg_result *d_res,
+                             const double origin[3], const kicp_free_space_params &p, uint32_t nb) {
+    kicp_ctx *c = m->ctx;
+    KICP_TRY(free_reserve(m));
+    KICP_CUDA(cudaMemsetAsync(m->d_free_stats, 0, kFreeStatWords * sizeof(unsigned long long) + (size_t)nb * sizeof(uint32_t), c->stream));
+    Pose pose{0, 0, 0, 1, 0, 0, 0};
+    if (pose7) pose = Pose{pose7[0], pose7[1], pose7[2], pose7[3], pose7[4], pose7[5], pose7[6]};
+    const FreeRayArgs a{origin[0], origin[1], origin[2], p.end_margin, m->max_distance, (uint32_t)p.min_misses};
+    const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)m->ctx->sm_count * 8));
+    k_free_rays<<<grid, 256, 0, c->stream>>>(m->view(), d_xyz, n, d_n, pose, d_res, a, m->d_free_flags, m->d_free_stats);
+    KICP_CHECK_LAUNCH(c);
+    return KICP_OK;
+}
+
+static int enqueue_mark_free(kicp_map *m, uint32_t nb, uint32_t min_misses, const kicp_reg_result *d_res) {
+    kicp_ctx *c = m->ctx;
+    k_mark_free<<<(nb + 255) / 256, 256, 0, c->stream>>>(m->blk, nb, m->prior_blocks, m->d_free_flags, min_misses, m->d_keep,
+                                                        m->d_counters, m->d_free_stats, d_res);
+    KICP_CHECK_LAUNCH(c);
+    return KICP_OK;
+}
+
 // RemovePointsFarFromLocation over the first `nb` blocks: k_mark_far flags the survivors, which are compacted (order kept) into the
 // spare arrays; those swap with the live ones and the table is rebuilt.  Synchronous (`d_res` null): the eviction zeroes the
 // counters, reads them back after k_mark_far and compacts only when a voxel died.  Frame path: the origin and the registration's
@@ -587,7 +630,22 @@ static int map_insert(kicp_map *m, const double *xyz, bool xyz_on_device, int64_
 // With a frozen prior of P blocks every step runs over the suffix [P, nb) only: the prior never dies, the spare arrays already hold
 // its copy at [0, P), and the table is restored from the prior's snapshot before the live blocks are re-inserted.  Each step is still
 // one launch.
-static int map_evict(kicp_map *m, const double origin[3], const kicp_reg_result *d_res, uint32_t nb) {
+// The survivors of d_keep over [P, nb) compacted in order into the spare arrays, which swap with the live ones; the host mirrors from
+// `res` (synchronous: the counters read back) and the table restored after the compaction
+static int map_compact(kicp_map *m, const kicp_reg_result *d_res, uint32_t nb, const uint32_t *res) {
+    kicp_ctx *c = m->ctx;
+    const uint32_t P = m->prior_blocks, nl = nb - P;
+    KICP_TRY(enqueue_exclusive_sum(c, m->d_keep + P, m->d_new_id + P, nl));
+    k_compact_blocks<<<(unsigned)(((uint64_t)nl * 32 + 255) / 256), 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, nb, m->d_keep,
+                                                                                       m->d_new_id, m->blk_spare, m->pts_spare, P);
+    KICP_CHECK_LAUNCH(c);
+    std::swap(m->blk, m->blk_spare);
+    std::swap(m->pts, m->pts_spare);
+    if (!d_res) KICP_TRY(kicp_map_finish_update(m, res, true));
+    return map_rebuild_table(m, m->nslots, d_res ? nb : m->num_blocks, d_res ? m->d_counters : nullptr, true);
+}
+// `free_min` (frame path with free-space clearing, > 0): k_mark_free runs after k_mark_far over the flags k_free_rays left
+static int map_evict(kicp_map *m, const double origin[3], const kicp_reg_result *d_res, uint32_t nb, uint32_t free_min = 0) {
     kicp_ctx *c = m->ctx;
     const uint32_t P = m->prior_blocks;
     if (nb <= P) return KICP_OK;  // (synchronous only: the frame path's bound exceeds the block count) nothing can die
@@ -597,21 +655,14 @@ static int map_evict(kicp_map *m, const double origin[3], const kicp_reg_result 
     k_mark_far<<<(nl + 255) / 256, 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, nb, origin[0], origin[1], origin[2],
                                                        m->max_distance * m->max_distance, m->d_keep, m->d_counters, d_res, P);
     KICP_CHECK_LAUNCH(c);
+    if (free_min) KICP_TRY(enqueue_mark_free(m, nb, free_min, d_res));
     uint32_t res[8];
     if (!d_res) {
         KICP_CUDA(cudaMemcpyAsync(res, m->d_counters, sizeof(res), cudaMemcpyDeviceToHost, c->stream));
         KICP_CUDA(cudaStreamSynchronize(c->stream));
         if (res[4] == 0) return KICP_OK;
     }
-    KICP_TRY(enqueue_exclusive_sum(c, m->d_keep + P, m->d_new_id + P, nl));
-    k_compact_blocks<<<(unsigned)(((uint64_t)nl * 32 + 255) / 256), 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, nb, m->d_keep,
-                                                                                       m->d_new_id, m->blk_spare, m->pts_spare, P);
-    KICP_CHECK_LAUNCH(c);
-    std::swap(m->blk, m->blk_spare);
-    std::swap(m->pts, m->pts_spare);
-    if (!d_res) KICP_TRY(kicp_map_finish_update(m, res, true));
-    // after the compaction
-    return map_rebuild_table(m, m->nslots, d_res ? nb : m->num_blocks, d_res ? m->d_counters : nullptr, true);
+    return map_compact(m, d_res, nb, res);
 }
 
 // AddPoints with the count and the pose on the host: one synchronisation, after which the host mirrors are current
@@ -699,15 +750,92 @@ extern "C" int kicp_map_update_pose_device(kicp_map *m, const void *data, int64_
 // still being computed on the stream: everything is enqueued, nothing is read back.  The counters are copied to `h_counters`
 // (pinned, 8 words); after the caller's end-of-frame synchronisation, kicp_map_finish_update() brings the host mirrors up to date.
 int kicp_map_update_pose_async(kicp_map *m, const double *d_xyz, int64_t n_max, const int *d_n, const kicp_reg_result *d_res,
-                               uint32_t *h_counters) {
-    if (!m || n_max <= 0 || !d_xyz || !d_n || !d_res || !h_counters) return KICP_ERR_INVALID;
+                               uint32_t *h_counters, const kicp_free_space_params *fs, const double fs_origin[3],
+                               kicp_free_space_stats *h_fs) {
+    if (!m || n_max <= 0 || !d_xyz || !d_n || !d_res || !h_counters || (fs && (!fs_origin || !h_fs))) return KICP_ERR_INVALID;
     KICP_TRY(map_insert(m, d_xyz, true, n_max, nullptr, d_n, d_res));
     // RemovePointsFarFromLocation(pose.translation()) over the blocks that exist now: at most ub
     const uint32_t ub = (uint32_t)std::min<uint64_t>((uint64_t)m->num_blocks + (uint64_t)n_max, m->blocks_cap);
+    // free-space clearing: the frame's rays against the map after the insert, decided after the eviction
+    if (fs) KICP_TRY(enqueue_free_rays(m, d_xyz, n_max, d_n, nullptr, d_res, fs_origin, *fs, ub));
     const double unused[3] = {0.0, 0.0, 0.0};
-    KICP_TRY(map_evict(m, unused, d_res, ub));
+    KICP_TRY(map_evict(m, unused, d_res, ub, fs ? (uint32_t)fs->min_misses : 0u));
     KICP_CUDA(cudaMemcpyAsync(h_counters, m->d_counters, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, m->ctx->stream));
+    static_assert(sizeof(kicp_free_space_stats) <= kFreeStatWords * sizeof(unsigned long long), "statistics words");
+    if (fs) KICP_CUDA(cudaMemcpyAsync(h_fs, m->d_free_stats, sizeof(kicp_free_space_stats), cudaMemcpyDeviceToHost, m->ctx->stream));
     return KICP_OK;
+}
+
+// Free-space clearing of the n rays of d_xyz (packed doubles in HBM, valid until the call returns) at a host pose, synchronously: the
+// flags, k_free_rays and k_mark_free, ONE read-back of the counters and the statistics, and (when a live voxel was cleared) the
+// eviction's compaction and table restore.  The host mirrors are current when it returns.
+int kicp_map_clear_free_space_packed(kicp_map *m, const double *d_xyz, int64_t n, const double pose[7], const double origin[3],
+                                     const kicp_free_space_params *p, kicp_free_space_stats *stats) {
+    kicp_ctx *c = m->ctx;
+    KICP_CUDA(cudaSetDevice(c->device));
+    kicp_free_space_stats st{};
+    if (n > 0) {
+        const uint32_t nb = m->num_blocks;
+        const uint32_t init[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        KICP_CUDA(cudaMemcpyAsync(m->d_counters, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
+        KICP_TRY(enqueue_free_rays(m, d_xyz, n, nullptr, pose, nullptr, origin, *p, nb));
+        if (nb) KICP_TRY(enqueue_mark_free(m, nb, (uint32_t)p->min_misses, nullptr));
+        uint32_t res[8];
+        KICP_CUDA(cudaMemcpyAsync(res, m->d_counters, sizeof(res), cudaMemcpyDeviceToHost, c->stream));
+        KICP_CUDA(cudaMemcpyAsync(&st, m->d_free_stats, sizeof(st), cudaMemcpyDeviceToHost, c->stream));
+        KICP_CUDA(cudaStreamSynchronize(c->stream));
+        if (res[4]) KICP_TRY(map_compact(m, nullptr, nb, res));
+    }
+    if (stats) *stats = st;
+    return KICP_OK;
+}
+
+// the checks of the clearing calls after their cloud's: pose, origin and parameters, the map last
+static int free_space_args(kicp_map *m, const char *fn, const double *pose, const double *origin, const kicp_free_space_params *p) {
+    if (!pose) return kicp_invalid(fn, "pose: null pointer");
+    if (!origin) return kicp_invalid(fn, "sensor_origin: null pointer");
+    if (!p) return kicp_invalid(fn, "params: null pointer");
+    for (int k = 0; k < 7; ++k)
+        if (!std::isfinite(pose[k])) return kicp_invalid(fn, "pose: not finite");
+    for (int k = 0; k < 3; ++k)
+        if (!std::isfinite(origin[k])) return kicp_invalid(fn, "sensor_origin: not finite");
+    KICP_TRY(kicp_check_free_space_params(fn, p, false));
+    if (!m) return kicp_invalid(fn, "null map");
+    return KICP_OK;
+}
+int kicp_check_free_space_params(const char *fn, const kicp_free_space_params *p, bool allow_off) {
+    if (!(p->end_margin >= 0.0) || std::isinf(p->end_margin)) return kicp_invalid(fn, "params->end_margin: NaN, negative or infinite");
+    if (p->min_misses < (allow_off ? 0 : 1)) return kicp_invalid(fn, allow_off ? "params->min_misses: negative" : "params->min_misses: < 1");
+    return KICP_OK;
+}
+
+extern "C" int kicp_map_clear_free_space(kicp_map *m, const double *xyz, int64_t n, const double pose[7], const double sensor_origin[3],
+                                         const kicp_free_space_params *params, kicp_free_space_stats *stats) {
+    static const char fn[] = "kicp_map_clear_free_space";
+    if (n < 0) return kicp_invalid(fn, "n < 0");
+    if (n >= (1ll << 40)) return kicp_invalid(fn, "n: 2^40 points or more");
+    if (n > 0 && !xyz) return kicp_invalid(fn, "xyz: null pointer");
+    KICP_TRY(free_space_args(m, fn, pose, sensor_origin, params));
+    KICP_CUDA(cudaSetDevice(m->ctx->device));
+    if (n > 0) {
+        KICP_TRY(map_reserve_input(m, n));
+        KICP_CUDA(cudaMemcpyAsync(m->d_in, xyz, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, m->ctx->stream));
+    }
+    return kicp_map_clear_free_space_packed(m, m->d_in, n, pose, sensor_origin, params, stats);
+}
+
+extern "C" int kicp_map_clear_free_space_device(kicp_map *m, const void *data, int64_t n, int32_t dtype, int32_t point_step, int32_t offset_x,
+                                                int32_t offset_y, int32_t offset_z, const double pose[7], const double sensor_origin[3],
+                                                const kicp_free_space_params *params, kicp_free_space_stats *stats) {
+    static const char fn[] = "kicp_map_clear_free_space_device";
+    const kicp_frame_input in{data, n, dtype, point_step, offset_x, offset_y, offset_z, nullptr, 0};
+    KICP_TRY(kicp_check_cloud_args(&in, fn));
+    KICP_TRY(free_space_args(m, fn, pose, sensor_origin, params));
+    bool packed = false;
+    KICP_TRY(kicp_check_device_cloud(m->ctx, &in, fn, &packed));
+    const double *xyz = nullptr;
+    KICP_TRY(map_device_points(m, in, packed, &xyz));
+    return kicp_map_clear_free_space_packed(m, xyz, n, pose, sensor_origin, params, stats);
 }
 
 // Pointcloud / export: the stored points are packed ON THE DEVICE (k_block_counts + k_exclusive_sum + k_pack_points, block order,

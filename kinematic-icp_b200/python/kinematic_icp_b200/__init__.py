@@ -24,7 +24,12 @@ __all__ = ["Context", "VoxelHashMap", "Scan", "KinematicRegistration", "KicpErro
            "RegisterFrame", "StageFrame", "StageLaserScan", "RegisterStagedFrame", "StagedFrame", "frame_clouds_f32",
            "frame_clouds_device", "PointCloudSensor", "LaserScanSensor", "StageSensors", "StagedSensors", "RegisterStagedSensors",
            "RegisterStagedFrameSegments", "RegisterStagedSensorsSegments", "deskew_segments", "CorrespondenceStats",
-           "frame_correspondences", "frame_correspondences_device", "PoseHypothesis", "PlanarAlignment", "frame_map_update"]
+           "frame_correspondences", "frame_correspondences_device", "PoseHypothesis", "PlanarAlignment", "frame_map_update",
+           "FreeSpaceStats", "frame_free_space", "FREE_SPACE_MIN_MISSES", "FREE_SPACE_END_MARGIN"]
+
+# The defaults of free-space clearing (VoxelHashMap.ClearFreeSpace, Context.set_free_space): see README, "Clearing free space"
+FREE_SPACE_MIN_MISSES = 2
+FREE_SPACE_END_MARGIN = 0.5
 
 
 class CorrespondenceStats(NamedTuple):
@@ -42,6 +47,20 @@ class CorrespondenceStats(NamedTuple):
     def from_c(cls, st):
         return cls(int(st.n_points), int(st.n_inliers), float(st.fitness), float(st.inlier_rmse), float(st.sum_sq), tuple(st.jtj),
                    tuple(st.jtr))
+
+
+class FreeSpaceStats(NamedTuple):
+    """kicp_free_space_stats: the rays cast, the voxels visited summed over them, the live voxels and points cleared, and the prior
+    voxels that met the clearing condition and were kept."""
+    rays: int
+    visits: int
+    cleared_voxels: int
+    cleared_points: int
+    prior_contradicted: int
+
+    @classmethod
+    def from_c(cls, st):
+        return cls(int(st.rays), int(st.visits), int(st.cleared_voxels), int(st.cleared_points), int(st.prior_contradicted))
 
 
 class PoseHypothesis(NamedTuple):
@@ -113,6 +132,13 @@ class Context:
         empty).  frame_map_update(ctx) tells what the last frame did."""
         p = _capi.MapUpdatePolicy(int(mode), int(min_inliers), float(min_fitness), float(max_inlier_rmse))
         check(lib().kicp_ctx_set_map_update(self.h, C.byref(p)), "kicp_ctx_set_map_update")
+
+    def set_free_space(self, min_misses=0, end_margin=0.0):
+        """kicp_ctx_set_free_space: with min_misses >= 1 the single-sensor frame calls clear free space after every applied Update (the
+        rule of VoxelHashMap.ClearFreeSpace on frame_downsample, from lidar_to_base's translation); 0 turns it off.  The multi-sensor
+        frame calls refuse to run while it is on.  frame_free_space(ctx) returns the last frame's statistics."""
+        p = _capi.FreeSpaceParams(float(end_margin), int(min_misses))
+        check(lib().kicp_ctx_set_free_space(self.h, C.byref(p)), "kicp_ctx_set_free_space")
 
     def wait_stream(self, stream):
         """kicp_ctx_wait_stream: the context's later work waits for everything enqueued on `stream` (a cudaStream_t int) so far."""
@@ -303,6 +329,27 @@ class VoxelHashMap:
             check(lib().kicp_map_update(self.h, dp(points), len(points), dp(a)), "kicp_map_update")
         else:
             check(lib().kicp_map_update_pose(self.h, dp(points), len(points), dp(a)), "kicp_map_update_pose")
+
+    def ClearFreeSpace(self, points, pose, sensor_origin=(0.0, 0.0, 0.0), *, min_misses=FREE_SPACE_MIN_MISSES,
+                       end_margin=FREE_SPACE_END_MARGIN, stream=None, point_step=0, offsets=(0, 0, 0)):
+        """Free-space clearing (kicp_map_clear_free_space): every point of `points` (frame F) is a ray from T * sensor_origin to
+        T * p, T = pose (F -> map).  A live voxel that at least `min_misses` rays pass through (each ray cut `end_margin` metres short of
+        its end and at max_distance) and in which no ray ends leaves the map; prior voxels are kept and counted.  Returns FreeSpaceStats.
+        A device cloud is taken as AddPoints takes it (kicp_map_clear_free_space_device).  The call returns when the map is updated."""
+        pose = as_pose(pose)
+        o = np.ascontiguousarray(sensor_origin, dtype=np.float64).reshape(3)
+        p = _capi.FreeSpaceParams(float(end_margin), int(min_misses))
+        st = _capi.FreeSpaceStats()
+        if _device.is_device(points):
+            d = self._device_points(points, stream, point_step, offsets)
+            check(lib().kicp_map_clear_free_space_device(self.h, d.ptr, d.n, d.dtype, d.point_step, *d.offsets, dp(pose), dp(o), C.byref(p),
+                                                         C.byref(st)), "kicp_map_clear_free_space_device")
+        else:
+            _host_only("ClearFreeSpace", stream=stream, point_step=point_step)
+            q = as_points(points) if len(points) else np.zeros((0, 3))
+            check(lib().kicp_map_clear_free_space(self.h, dp(q), len(q), dp(pose), dp(o), C.byref(p), C.byref(st)),
+                  "kicp_map_clear_free_space")
+        return FreeSpaceStats.from_c(st)
 
     def freeze(self):
         """kicp_map_freeze: every voxel now in the map becomes a read-only prior that Update never evicts and AddPoints never writes
@@ -546,6 +593,14 @@ def frame_map_update(ctx):
     o = C.c_int32()
     check(lib().kicp_frame_map_update(ctx.h, C.byref(o)), "kicp_frame_map_update")
     return int(o.value)
+
+
+def frame_free_space(ctx):
+    """FreeSpaceStats of the last frame call on `ctx` (kicp_frame_free_space): all zero when the option was off, the Update was not
+    applied or the frame failed."""
+    st = _capi.FreeSpaceStats()
+    check(lib().kicp_frame_free_space(ctx.h, C.byref(st)), "kicp_frame_free_space")
+    return FreeSpaceStats.from_c(st)
 
 
 def frame_correspondences_device(ctx):

@@ -92,6 +92,17 @@ class MapUpdatePolicy(C.Structure):
     _fields_ = [("mode", C.c_int32), ("min_inliers", C.c_int64), ("min_fitness", C.c_double), ("max_inlier_rmse", C.c_double)]
 
 
+class FreeSpaceParams(C.Structure):
+    """kicp_free_space_params"""
+    _fields_ = [("end_margin", C.c_double), ("min_misses", C.c_int32)]
+
+
+class FreeSpaceStats(C.Structure):
+    """kicp_free_space_stats"""
+    _fields_ = [("rays", C.c_int64), ("visits", C.c_int64), ("cleared_voxels", C.c_int64), ("cleared_points", C.c_int64),
+                ("prior_contradicted", C.c_int64)]
+
+
 class FrameInput(C.Structure):
     """kicp_frame_input"""
     _fields_ = [("data", C.c_void_p), ("n", C.c_int64), ("dtype", C.c_int32), ("point_step", C.c_int32), ("offset_x", C.c_int32),
@@ -184,6 +195,9 @@ SYMBOLS = [
     ("kicp_map_prior_size", C.c_int, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     ("kicp_map_pointcloud_layer", C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
     ("kicp_map_pointcloud_layer_device_async", C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
+    ("kicp_map_clear_free_space", C.c_int, [_P, c_dp, C.c_int64, c_dp, c_dp, C.POINTER(FreeSpaceParams), C.POINTER(FreeSpaceStats)]),
+    ("kicp_map_clear_free_space_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp, c_dp,
+                                                   C.POINTER(FreeSpaceParams), C.POINTER(FreeSpaceStats)]),
     ("kicp_map_nearest", C.c_int, [_P, c_dp, C.c_int64, c_dp, c_dp]),
     ("kicp_map_add_points_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     ("kicp_map_update_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp]),
@@ -228,6 +242,8 @@ SYMBOLS = [
     ("kicp_frame_correspondences_device", C.c_int, [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_int64)]),
     ("kicp_ctx_set_map_update", C.c_int, [_P, C.POINTER(MapUpdatePolicy)]),
     ("kicp_frame_map_update", C.c_int, [_P, C.POINTER(C.c_int32)]),
+    ("kicp_ctx_set_free_space", C.c_int, [_P, C.POINTER(FreeSpaceParams)]),
+    ("kicp_frame_free_space", C.c_int, [_P, C.POINTER(FreeSpaceStats)]),
     ("kicp_frame_stage", C.c_int, [_P, C.POINTER(FrameInput), C.c_int32, C.c_int32, c_dp, C.POINTER(C.c_int64)]),
     ("kicp_frame_stage_device", C.c_int, [_P, C.POINTER(FrameInput), C.c_int32, C.c_int32, c_dp, C.POINTER(C.c_int64)]),
     ("kicp_register_staged_frame", C.c_int, [_P, c_dp, c_dp, c_dp, c_dp, C.c_double, C.POINTER(FrameParams), c_dp, c_dp, C.c_int64,
