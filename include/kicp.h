@@ -238,8 +238,8 @@ int kicp_map_pointcloud_layer_device_async(kicp_map *map, int32_t layer, int32_t
  *      d_j == 0: tmax_j = +inf (k_j + 1 and k_j * v in double).  Visit k; then at most |K(q_i) - K(o)|_1 times: take the axis j of the
  *      smallest tmax (the lowest index on ties), stop if tmax_j >= t_end, else k_j += step_j, tmax_j += tdelta_j and visit k.  A visited
  *      voxel that is in the map and is not K(q_i) gets one miss from this ray.
- *   5. Decision: a LIVE voxel (block index >= P) with at least min_misses misses and no hit is cleared.  A prior voxel that meets the
- *      condition is kept (prior voxels are read-only, kicp_map_freeze) and counted in prior_contradicted: its prior is going stale.
+ *   5. Decision (occupancy off; kicp_map_set_occupancy below keeps evidence across calls): a LIVE voxel (block index >= P) with at
+ *      least min_misses misses and no hit is cleared.  A prior voxel that meets the condition is kept (prior voxels are read-only, kicp_map_freeze) and counted in prior_contradicted: its prior is going stale.
  *   6. Removal: cleared voxels leave through the eviction's stable compaction; the survivors keep their relative order, so the exports
  *      after the call are determined bit for bit.
  *      The result depends only on integer counts: not on the order of the rays or on the launch shape.
@@ -267,6 +267,39 @@ int kicp_map_clear_free_space(kicp_map *map, const double *xyz, int64_t n, const
 int kicp_map_clear_free_space_device(kicp_map *map, const void *data, int64_t n, int32_t dtype, int32_t point_step, int32_t offset_x,
                                      int32_t offset_y, int32_t offset_z, const double pose[7], const double sensor_origin[3],
                                      const kicp_free_space_params *params, kicp_free_space_stats *stats);
+/* ---- occupancy evidence: a setting of the MAP (not of the context: the evidence is map state and survives evictions, growth and
+ *      freezes) that gives step 5 above a memory across clearing calls.  One clearing call is kicp_map_clear_free_space[_device] or
+ *      the frame path's clearing after an applied Update (kicp_ctx_set_free_space); steps 1-4 give every voxel b its hit_b and miss_b,
+ *      and free_b = !hit_b && miss_b >= min_misses is the condition of step 5.
+ *   Off (the default, or after kicp_map_set_occupancy(map, NULL)): step 5 as above.
+ *   On: every LIVE voxel (block index >= P) carries an int32 evidence e_b, updated once per clearing call:
+ *     hit_b:  e_b = min(e_b + hit_gain, max_evidence);
+ *     else free_b: e_b = e_b - miss_loss, and the voxel is cleared when e_b <= 0 (it leaves through step 6 and is counted in
+ *             cleared_voxels / cleared_points);
+ *     else:   unchanged.
+ *   Prior voxels keep their evidence while frozen; prior_contradicted counts free_b as above.  A voxel gets `initial` when an insert
+ *   creates it (every AddPoints / Update variant and the frame path), when kicp_map_load_voxels loads it, and when it is in the map at
+ *   a kicp_map_set_occupancy call (every set call resets all voxels to `initial`); a voxel evicted by distance and created again starts
+ *   again at `initial`.  kicp_map_freeze freezes the prior voxels' evidence with them and kicp_map_thaw resumes it; kicp_map_clear (and
+ *   the facade's SetPose) empties the map and keeps the setting.  Only clearing calls change evidence: an Update without clearing
+ *   leaves it alone, and a node that clears once per sensor updates it once per such call.  The result depends only on integer counts
+ *   (not on ray order or launch shape), and {1, 0, 1, 1} gives the memoryless rule's exports and statistics byte for byte.
+ *   Cost: two int32 per block of capacity (the evidence and its compaction target), allocated by the set call; no extra launch in the
+ *   clearing calls or the inserts (kicp_map_load_voxels adds one fill). -------------------------------------------------------------- */
+typedef struct kicp_occupancy_params {
+    int32_t initial;      /* evidence of a new voxel: 1 <= initial <= max_evidence */
+    int32_t hit_gain;     /* added when a ray ends in the voxel: 0 <= hit_gain <= 2^24 */
+    int32_t miss_loss;    /* subtracted when the voxel is free in a call: 1 <= miss_loss <= 2^24 */
+    int32_t max_evidence; /* the cap of the evidence: max_evidence <= 2^24 (with these bounds int32 arithmetic cannot overflow) */
+} kicp_occupancy_params;
+/* Turns occupancy on with `params` (every voxel now in the map, prior included, starts at params->initial) or off with NULL (the
+ * arrays are freed).  Synchronous.  Errors: KICP_ERR_INVALID, with kicp_last_error naming the field, for a value out of range, or a
+ * null map; the previous setting is kept. */
+int kicp_map_set_occupancy(kicp_map *map, const kicp_occupancy_params *params);
+/* The evidence of every voxel in kicp_map_export_voxels' block order (prior first): *n = the voxel count, then n int32 copied to
+ * `evidence` with one host synchronisation.  Errors: KICP_ERR_INVALID when occupancy is off or for a null map or n (evidence may be
+ * NULL when the map is empty), KICP_ERR_CAPACITY when cap < *n (nothing copied). */
+int kicp_map_export_occupancy(kicp_map *map, int32_t *evidence, int64_t cap, int64_t *n);
 /* GetClosestNeighbor(query) for n queries: (closest point, distance); (0,0,0), DBL_MAX when nothing is found. */
 int kicp_map_nearest(kicp_map *map, const double *queries, int64_t n, double *out_points, double *out_dist);
 /* ---- the map operators on clouds in device memory.  `data` holds n points of device memory of the context's device in the layout of

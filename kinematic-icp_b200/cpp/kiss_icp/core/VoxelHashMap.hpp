@@ -79,6 +79,23 @@ struct VoxelHashMap {
                     "kicp_map_clear_free_space");
         return st;
     }
+    // the defaults of occupancy evidence (README, "Clearing free space"; the Python OCCUPANCY_* constants)
+    static constexpr kicp_occupancy_params kDefaultOccupancy{3, 1, 1, 3};
+    // Occupancy evidence of the clearing calls (kicp_map_set_occupancy): a live voxel keeps an integer evidence across calls and is
+    // cleared when it reaches 0; nullptr turns it off.  A setting of the map: Clear() (and so KinematicICP::SetPose) keeps it.  The
+    // pipeline reaches it through KinematicICP::VoxelMap().  Throws on an error (a field out of range is named).
+    void SetOccupancy(const kicp_occupancy_params *params) {
+        kicp::check(kicp_map_set_occupancy(handle_, params), "kicp_map_set_occupancy");
+    }
+    // the evidence of every voxel in the block order of kicp_map_export_voxels (prior first); throws when occupancy is off
+    std::vector<int32_t> Occupancy() const {
+        int64_t n = 0;
+        kicp::check(kicp_map_num_voxels(handle_, &n), "kicp_map_num_voxels");
+        std::vector<int32_t> out(static_cast<size_t>(n));
+        kicp::check(kicp_map_export_occupancy(handle_, out.data(), n, &n), "kicp_map_export_occupancy");
+        out.resize(static_cast<size_t>(n));
+        return out;
+    }
     void AddPoints(const std::vector<Eigen::Vector3d> &points) {
         kicp::check(kicp_map_add_points(handle_, kicp::xyz(points), (int64_t)points.size()), "kicp_map_add_points");
     }

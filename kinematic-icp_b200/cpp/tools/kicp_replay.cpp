@@ -57,6 +57,10 @@
 // down-sampled points clear the live voxels their rays pass through.  The JSON line then reports "free_space" {min_misses,
 // end_margin} and the statistics summed over the last repetition's frames ("free_space_stats": rays, visits, cleared_voxels,
 // cleared_points, prior_contradicted).  A multi-sensor (KSEQ3 with several slots) drive is refused with it.
+// --occupancy I,G,L,M (needs --free-space) keeps occupancy evidence in the pipeline's map (kicp.h kicp_map_set_occupancy, set through
+// KinematicICP::VoxelMap() after the map is loaded): initial I, hit_gain G, miss_loss L, max_evidence M.  The JSON line then reports
+// "occupancy" {initial, hit_gain, miss_loss, max_evidence, voxels, evidence_sum}: the setting, and the map's voxel count and summed
+// evidence at the end of the last repetition.
 //
 // Version 3, magic "KSEQ3\0\0\0", carries several message streams ("slots", 1..KICP_MAX_SENSORS: PointCloud2 records or 2D LaserScans,
 // each with its extrinsic) and the wheel odometry either as one relative motion or as poses sampled during the sweep:
@@ -235,7 +239,7 @@ int main(int argc, char **argv) {
         std::fprintf(stderr, "usage: %s drive.kseq out.tum [--deskew 0|1] [--voxel-size v] [--max-range r] [--min-range r] [--repeat k] [--pageable] "
                      "[--host-stamps] [--device-input] [--publish host|device|live] [--publish-digest FILE] [--downsample-order 0|1] "
                      "[--correspondences FILE] [--map-update always|never|gated] [--min-inliers k] [--min-fitness f] [--max-inlier-rmse r] "
-                     "[--load-map FILE] [--freeze-prior] [--save-map FILE] [--free-space M[,E]]\n", argv[0]);
+                     "[--load-map FILE] [--freeze-prior] [--save-map FILE] [--free-space M[,E]] [--occupancy I,G,L,M]\n", argv[0]);
         return 2;
     }
     kinematic_icp::pipeline::Config config;  // the reference's defaults (pipeline/KinematicICP.hpp:38-60)
@@ -248,6 +252,8 @@ int main(int argc, char **argv) {
     kicp_map_update_policy policy{KICP_MAP_UPDATE_ALWAYS, 0, 0.0, HUGE_VAL};
     bool freeze_prior = false;  // --freeze-prior: freeze the map --load-map loaded
     kicp_free_space_params free_space{0.5, 0};  // --free-space M[,E]; min_misses 0: off
+    bool occupancy = false;  // --occupancy I,G,L,M
+    kicp_occupancy_params occ{0, 0, 0, 0};
     bool thresholds = false;  // a --min-* / --max-inlier-rmse option was given (only with --map-update gated)
     bool map_options = false;  // any of --map-update, the thresholds, --load-map, --save-map: the JSON line reports the outcomes
     for (int i = 3; i < argc; ++i) {
@@ -290,6 +296,19 @@ int main(int argc, char **argv) {
                         throw std::runtime_error("--free-space takes M[,E]: min_misses M >= 1, end_margin E >= 0 metres");
                 }
             }
+            else if (a == "--occupancy") {
+                const std::string v = value("--occupancy");
+                int32_t f[4];
+                const char *q = v.c_str();
+                for (int k = 0; k < 4; ++k) {
+                    char *end = nullptr;
+                    const long x = std::strtol(q, &end, 10);
+                    if (end == q || x < INT32_MIN || x > INT32_MAX || *end != (k < 3 ? ',' : '\0'))
+                        throw std::runtime_error("--occupancy takes I,G,L,M: initial, hit_gain, miss_loss, max_evidence (integers)");
+                    f[k] = (int32_t)x, q = end + 1;
+                }
+                occ = kicp_occupancy_params{f[0], f[1], f[2], f[3]}, occupancy = true;
+            }
             else if (a == "--downsample-order") {
                 const std::string v = value("--downsample-order");
                 if (v != "0" && v != "1") throw std::runtime_error("--downsample-order takes 0 or 1");
@@ -311,6 +330,10 @@ int main(int argc, char **argv) {
     }
     if (freeze_prior && load_map_path.empty()) {
         std::fprintf(stderr, "kicp_replay: --freeze-prior freezes the map --load-map loads: it needs --load-map\n");
+        return 2;
+    }
+    if (occupancy && free_space.min_misses == 0) {
+        std::fprintf(stderr, "kicp_replay: --occupancy keeps evidence across the frames' free-space clearing: it needs --free-space\n");
         return 2;
     }
     map_options = map_options || thresholds;
@@ -418,6 +441,7 @@ int main(int argc, char **argv) {
         double map_seconds = 0.0;  // --publish, last repetition: time spent publishing the local map
         int64_t outcomes[KICP_FRAME_UPDATE_NONE + 1] = {};  // frames of the last repetition per KICP_FRAME_UPDATE_* outcome
         kicp_free_space_stats free_sum{};  // --free-space: the statistics summed over the last repetition's frames
+        int64_t occ_voxels = 0, occ_sum = 0;  // --occupancy: the map's voxels and summed evidence after the last repetition
         std::vector<double> rep_seconds;  // every repetition's wall time (a 24-frame drive lasts milliseconds: one hiccup halves a single figure)
         for (int rep = 0; rep < repeat; ++rep) {  // --repeat: the same drive again on a fresh pipeline (the last run is the one written)
             kinematic_icp::pipeline::KinematicICP pipeline(config);
@@ -427,6 +451,7 @@ int main(int argc, char **argv) {
                                                  prior.num_voxels()),
                             "kicp_map_load_voxels");
             if (freeze_prior) kicp::check(kicp_map_freeze(pipeline.VoxelMap().handle_), "kicp_map_freeze");
+            if (occupancy) pipeline.VoxelMap().SetOccupancy(&occ);  // a field out of range throws, naming it
             for (int64_t &o : outcomes) o = 0;
             free_sum = kicp_free_space_stats{};
             poses.clear();
@@ -539,6 +564,11 @@ int main(int argc, char **argv) {
             seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
             rep_seconds.push_back(seconds);
             kicp::check(kicp_map_num_points(pipeline.VoxelMap().handle_, &map_points), "kicp_map_num_points");
+            if (occupancy) {
+                const std::vector<int32_t> ev = pipeline.VoxelMap().Occupancy();
+                occ_voxels = (int64_t)ev.size(), occ_sum = 0;
+                for (const int32_t e : ev) occ_sum += e;
+            }
             if (freeze_prior) {
                 kicp::check(kicp_map_prior_size(pipeline.VoxelMap().handle_, &prior_voxels, &prior_points), "kicp_map_prior_size");
                 kicp::check(kicp_map_num_voxels(pipeline.VoxelMap().handle_, &map_voxels), "kicp_map_num_voxels");
@@ -616,6 +646,13 @@ int main(int argc, char **argv) {
                           "\"visits\": %lld, \"cleared_voxels\": %lld, \"cleared_points\": %lld, \"prior_contradicted\": %lld}",
                           (int)free_space.min_misses, free_space.end_margin, (long long)free_sum.rays, (long long)free_sum.visits,
                           (long long)free_sum.cleared_voxels, (long long)free_sum.cleared_points, (long long)free_sum.prior_contradicted);
+            live += buf;
+        }
+        if (occupancy) {
+            char buf[256];
+            std::snprintf(buf, sizeof(buf), ", \"occupancy\": {\"initial\": %d, \"hit_gain\": %d, \"miss_loss\": %d, \"max_evidence\": %d, "
+                          "\"voxels\": %lld, \"evidence_sum\": %lld}", (int)occ.initial, (int)occ.hit_gain, (int)occ.miss_loss,
+                          (int)occ.max_evidence, (long long)occ_voxels, (long long)occ_sum);
             live += buf;
         }
         if (v3) {  // the slots, their kinds, and the odometry samples per frame (0: one motion per frame)

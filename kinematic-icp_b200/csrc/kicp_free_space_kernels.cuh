@@ -121,13 +121,21 @@ __global__ void __launch_bounds__(256) k_free_rays(MapView m, const double *__re
     }
 }
 
+// Occupancy evidence (kicp_map_set_occupancy): the update of a live block's int32 evidence in a clearing call
+struct OccupancyArgs {
+    int32_t hit_gain, miss_loss, max_evidence;
+};
+
 // The decision over blocks [0, num_blocks): a block with at least min_misses misses and no hit is free.  A free prior block
 // (b < prior_blocks) is kept and counted in stats[4].  A free live block is cleared: keep[b] = 0, and it is counted in the words that
 // kicp_map_finish_update reads (counters[4] blocks, counters[d_res ? 5 : 3] points) and in stats[2] / stats[3].
 // Synchronous (`d_res` null): this kernel writes keep[b] for every live block.  Frame path (after k_mark_far): a block k_mark_far
 // already evicted stays evicted and is not counted here, and blocks beyond the insert's count (counters[0]) are skipped.
+// `evidence` (occupancy on): a live block's evidence gains hit_gain (up to max_evidence) on a hit and loses miss_loss when free; a free
+// block is cleared only when its evidence reaches 0 or less.  The prior's evidence is not touched.
 __global__ void k_mark_free(const int4 *blk, uint32_t num_blocks, uint32_t prior_blocks, const uint32_t *flags, uint32_t min_misses,
-                            uint32_t *keep, uint32_t *counters, unsigned long long *stats, const kicp_reg_result *d_res = nullptr) {
+                            uint32_t *keep, uint32_t *counters, unsigned long long *stats, const kicp_reg_result *d_res = nullptr,
+                            int32_t *evidence = nullptr, OccupancyArgs occ = OccupancyArgs{0, 0, 0}) {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= num_blocks) return;
     if (d_res && b >= counters[0]) return;
@@ -137,10 +145,23 @@ __global__ void k_mark_free(const int4 *blk, uint32_t num_blocks, uint32_t prior
         if (free) atomicAdd(&stats[4], 1ull);
         return;
     }
-    if (!d_res) keep[b] = free ? 0u : 1u;
-    else if (!free || !keep[b]) return;
+    if (d_res && !keep[b]) return;  // evicted by distance
+    bool clear = free;
+    if (evidence) {
+        // |e| <= 2^24 and gain, loss <= 2^24: no overflow
+        const int32_t e = evidence[b];
+        if (w & kFreeHit) {
+            const int32_t g = e + occ.hit_gain;
+            evidence[b] = g < occ.max_evidence ? g : occ.max_evidence;
+        } else if (free) {
+            evidence[b] = e - occ.miss_loss;
+            clear = e - occ.miss_loss <= 0;
+        }
+    }
+    if (!d_res) keep[b] = clear ? 0u : 1u;
+    else if (!clear) return;
     else keep[b] = 0u;
-    if (free) {
+    if (clear) {
         const uint32_t pts = (uint32_t)blk[b].w;
         atomicAdd(&counters[4], 1u);
         atomicAdd(&counters[d_res ? 5 : 3], pts);

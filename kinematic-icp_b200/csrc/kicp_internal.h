@@ -133,6 +133,11 @@ struct kicp_map {
     unsigned long long *d_free_stats = nullptr;
     uint32_t *d_free_flags = nullptr;
     uint32_t free_cap = 0;
+    // occupancy evidence (kicp_map_set_occupancy; null when off): one allocation (occ_slab) of 2 * occ_cap int32, the evidence of every
+    // block and the spare array a compaction writes into (swapped with it like blk / pts; while frozen it holds the prior's prefix too)
+    int32_t *occ_slab = nullptr, *d_occ = nullptr, *d_occ_spare = nullptr;
+    uint32_t occ_cap = 0;
+    kicp_occupancy_params occ = {0, 0, 0, 0};
     // state of kicp_map_pointcloud_f32_live (kicp_map.cu), created by its first call
     struct MapLive *live = nullptr;
     // correspondence report (kicp_map.cu, created by its first use): the per-CTA partials of k_corr_eval for corr_grid CTAs, the

@@ -329,6 +329,8 @@ static int map_mirror_prior(kicp_map *m) {
     KICP_CUDA(cudaMemcpyAsync(m->blk_spare, m->blk, (size_t)P * sizeof(int4), cudaMemcpyDeviceToDevice, c->stream));
     KICP_CUDA(cudaMemcpyAsync(m->pts_spare, m->pts, (size_t)P * m->cap * KICP_PSTRIDE * sizeof(double), cudaMemcpyDeviceToDevice,
                               c->stream));
+    if (m->d_occ)
+        KICP_CUDA(cudaMemcpyAsync(m->d_occ_spare, m->d_occ, (size_t)P * sizeof(int32_t), cudaMemcpyDeviceToDevice, c->stream));
     return KICP_OK;
 }
 
@@ -367,7 +369,22 @@ static int map_alloc_storage(kicp_map *m, uint32_t ncap) {
     }
     k_fill_i32<<<(ncap + 255) / 256, 256, 0, c->stream>>>(nhead, -1, ncap);
     KICP_CHECK_LAUNCH(c);
+    int32_t *nocc = nullptr;  // occupancy on: the evidence of [0, num_blocks) moves to a grown allocation
+    if (m->occ_slab) {
+        const cudaError_t e = cudaMalloc(&nocc, (size_t)2 * ncap * sizeof(int32_t));
+        if (e != cudaSuccess) {
+            cudaStreamSynchronize(c->stream);
+            cudaFree(slab);
+            return kicp_cuda_fail(e, "cudaMalloc", __FILE__, __LINE__);
+        }
+        if (m->num_blocks)
+            KICP_CUDA(cudaMemcpyAsync(nocc, m->d_occ, (size_t)m->num_blocks * sizeof(int32_t), cudaMemcpyDeviceToDevice, c->stream));
+    }
     KICP_CUDA(cudaStreamSynchronize(c->stream));
+    if (nocc) {
+        cudaFree(m->occ_slab);
+        m->occ_slab = m->d_occ = nocc, m->d_occ_spare = nocc + ncap, m->occ_cap = ncap;
+    }
     cudaFree(m->slab);
     m->slab = slab, m->slab_bytes = off;
     m->blk = nblk, m->pts = npts, m->pend_head = nhead, m->blocks_cap = ncap;
@@ -454,7 +471,7 @@ extern "C" int kicp_map_destroy(kicp_map *m) {
     if (!m) return KICP_OK;
     cudaSetDevice(m->ctx->device);
     cudaStreamSynchronize(m->ctx->stream);
-    cudaFree(m->slab), cudaFree(m->d_counters), cudaFree(m->d_free_stats);
+    cudaFree(m->slab), cudaFree(m->d_counters), cudaFree(m->d_free_stats), cudaFree(m->occ_slab);
     map_prior_free(m);
     cudaFree(m->d_in), cudaFree(m->d_xyz_t), cudaFree(m->d_next), cudaFree(m->d_touched), cudaFree(m->d_dist);
     cudaFree(m->d_corr_part), cudaFree(m->d_corr_stats), cudaFree(m->d_corr_inl);
@@ -569,7 +586,7 @@ static int map_insert(kicp_map *m, const double *xyz, bool xyz_on_device, int64_
     if (pose7) pose = Pose{pose7[0], pose7[1], pose7[2], pose7[3], pose7[4], pose7[5], pose7[6]};
     const unsigned grid = (unsigned)((n + 255) / 256);
     k_add_find_or_create<<<grid, 256, 0, c->stream>>>(rw, xyz, n, pose7 || d_res ? 1 : 0, pose, m->d_xyz_t, m->d_next, m->d_counters,
-                                                     m->d_touched, d_n, d_res, m->prior_blocks);
+                                                     m->d_touched, d_n, d_res, m->prior_blocks, m->d_occ, m->occ.initial);
     KICP_CHECK_LAUNCH(c);
     // KISS AddPoints: map_resolution = sqrt(voxel_size^2 / max_points_per_voxel)
     const double map_resolution = std::sqrt(m->voxel_size * m->voxel_size / (double)m->cap);
@@ -615,8 +632,9 @@ static int enqueue_free_rays(kicp_map *m, const double *d_xyz, int64_t n, const 
 
 static int enqueue_mark_free(kicp_map *m, uint32_t nb, uint32_t min_misses, const kicp_reg_result *d_res) {
     kicp_ctx *c = m->ctx;
+    const OccupancyArgs occ{m->occ.hit_gain, m->occ.miss_loss, m->occ.max_evidence};
     k_mark_free<<<(nb + 255) / 256, 256, 0, c->stream>>>(m->blk, nb, m->prior_blocks, m->d_free_flags, min_misses, m->d_keep,
-                                                        m->d_counters, m->d_free_stats, d_res);
+                                                        m->d_counters, m->d_free_stats, d_res, m->d_occ, occ);
     KICP_CHECK_LAUNCH(c);
     return KICP_OK;
 }
@@ -637,10 +655,12 @@ static int map_compact(kicp_map *m, const kicp_reg_result *d_res, uint32_t nb, c
     const uint32_t P = m->prior_blocks, nl = nb - P;
     KICP_TRY(enqueue_exclusive_sum(c, m->d_keep + P, m->d_new_id + P, nl));
     k_compact_blocks<<<(unsigned)(((uint64_t)nl * 32 + 255) / 256), 256, 0, c->stream>>>(m->blk, m->pts, (int)m->cap, nb, m->d_keep,
-                                                                                       m->d_new_id, m->blk_spare, m->pts_spare, P);
+                                                                                       m->d_new_id, m->blk_spare, m->pts_spare, P, m->d_occ,
+                                                                                       m->d_occ_spare);
     KICP_CHECK_LAUNCH(c);
     std::swap(m->blk, m->blk_spare);
     std::swap(m->pts, m->pts_spare);
+    std::swap(m->d_occ, m->d_occ_spare);
     if (!d_res) KICP_TRY(kicp_map_finish_update(m, res, true));
     return map_rebuild_table(m, m->nslots, d_res ? nb : m->num_blocks, d_res ? m->d_counters : nullptr, true);
 }
@@ -836,6 +856,52 @@ extern "C" int kicp_map_clear_free_space_device(kicp_map *m, const void *data, i
     const double *xyz = nullptr;
     KICP_TRY(map_device_points(m, in, packed, &xyz));
     return kicp_map_clear_free_space_packed(m, xyz, n, pose, sensor_origin, params, stats);
+}
+
+// ---------------------------------------------------------------------------------------------------- occupancy evidence
+// The setting of the map, checked field by field (the map last); a set call (re)allocates the evidence and its spare array for the
+// block capacity and fills both with `initial` (the spare's copy of a frozen prefix included); NULL frees them.
+extern "C" int kicp_map_set_occupancy(kicp_map *m, const kicp_occupancy_params *p) {
+    static const char fn[] = "kicp_map_set_occupancy";
+    constexpr int32_t kMax = 1 << 24;
+    if (p) {
+        if (p->max_evidence < 1 || p->max_evidence > kMax) return kicp_invalid(fn, "params->max_evidence: outside [1, 2^24]");
+        if (p->initial < 1 || p->initial > p->max_evidence) return kicp_invalid(fn, "params->initial: outside [1, max_evidence]");
+        if (p->hit_gain < 0 || p->hit_gain > kMax) return kicp_invalid(fn, "params->hit_gain: outside [0, 2^24]");
+        if (p->miss_loss < 1 || p->miss_loss > kMax) return kicp_invalid(fn, "params->miss_loss: outside [1, 2^24]");
+    }
+    if (!m) return kicp_invalid(fn, "null map");
+    kicp_ctx *c = m->ctx;
+    KICP_CUDA(cudaSetDevice(c->device));
+    KICP_CUDA(cudaStreamSynchronize(c->stream));
+    if (!p || m->occ_cap < m->blocks_cap) {
+        cudaFree(m->occ_slab);
+        m->occ_slab = m->d_occ = m->d_occ_spare = nullptr, m->occ_cap = 0, m->occ = kicp_occupancy_params{0, 0, 0, 0};
+        if (!p) return KICP_OK;
+        KICP_CUDA(cudaMalloc(&m->occ_slab, (size_t)2 * m->blocks_cap * sizeof(int32_t)));
+        m->occ_cap = m->blocks_cap;
+    }
+    m->d_occ = m->occ_slab, m->d_occ_spare = m->occ_slab + m->occ_cap;
+    k_fill_i32<<<(2 * m->occ_cap + 255) / 256, 256, 0, c->stream>>>(m->occ_slab, p->initial, 2 * m->occ_cap);
+    KICP_CHECK_LAUNCH(c);
+    m->occ = *p;
+    KICP_CUDA(cudaStreamSynchronize(c->stream));
+    return KICP_OK;
+}
+
+extern "C" int kicp_map_export_occupancy(kicp_map *m, int32_t *evidence, int64_t cap, int64_t *n) {
+    static const char fn[] = "kicp_map_export_occupancy";
+    if (!n) return kicp_invalid(fn, "n: null pointer");
+    if (!m) return kicp_invalid(fn, "null map");
+    if (!m->d_occ) return kicp_invalid(fn, "occupancy is off (kicp_map_set_occupancy)");
+    *n = m->num_blocks;
+    if (cap < *n) return KICP_ERR_CAPACITY;
+    if (*n == 0) return KICP_OK;
+    if (!evidence) return kicp_invalid(fn, "evidence: null pointer");
+    KICP_CUDA(cudaSetDevice(m->ctx->device));
+    KICP_CUDA(cudaMemcpyAsync(evidence, m->d_occ, (size_t)*n * sizeof(int32_t), cudaMemcpyDeviceToHost, m->ctx->stream));
+    KICP_CUDA(cudaStreamSynchronize(m->ctx->stream));
+    return KICP_OK;
 }
 
 // Pointcloud / export: the stored points are packed ON THE DEVICE (k_block_counts + k_exclusive_sum + k_pack_points, block order,
@@ -1148,6 +1214,10 @@ extern "C" int kicp_map_load_voxels(kicp_map *m, const int32_t *keys, const int3
     k_load_voxels<<<(unsigned)(((uint64_t)num_voxels * 32 + 255) / 256), 256, 0, c->stream>>>(
         m->blk, m->pts, (int)m->cap, d_keys, d_counts, d_off, d_pts, (uint32_t)num_voxels);
     KICP_CHECK_LAUNCH(c);
+    if (m->d_occ) {  // occupancy on: every loaded voxel starts at `initial`
+        k_fill_i32<<<(unsigned)((num_voxels + 255) / 256), 256, 0, c->stream>>>(m->d_occ, m->occ.initial, (uint32_t)num_voxels);
+        KICP_CHECK_LAUNCH(c);
+    }
     m->num_blocks = (uint32_t)num_voxels;
     m->num_points = total;
     int st = map_rebuild_table(m, m->nslots, m->num_blocks);

@@ -78,10 +78,11 @@ __global__ void k_table_rebuild(int4 *slots, uint32_t mask_in, const int4 *blk, 
 // block of the registration that precedes this launch on the stream) are read from device memory; a registration that did not
 // end with KICP_OK (NaN pose) leaves the map untouched.
 // `prior_blocks`: blocks [0, prior_blocks) are a frozen prior (kicp_map_freeze); a point whose voxel is one of them is dropped.
+// `evidence` (occupancy on, kicp_map_set_occupancy): a block this launch creates starts at `initial`.
 __global__ void k_add_find_or_create(MapRW m, const double *__restrict__ xyz, int64_t n, int has_pose, Pose pose,
                                      double *__restrict__ xyz_t, int32_t *__restrict__ pend_next, uint32_t *counters,
                                      int32_t *__restrict__ touched, const int *d_n = nullptr, const kicp_reg_result *d_res = nullptr,
-                                     uint32_t prior_blocks = 0) {
+                                     uint32_t prior_blocks = 0, int32_t *evidence = nullptr, int32_t initial = 0) {
     __shared__ uint32_t s_mask[32];
     const uint32_t tmask = lane_private(m.mask, s_mask);  // divergence safety, see kicp_device.cuh
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -114,6 +115,7 @@ __global__ void k_add_find_or_create(MapRW m, const double *__restrict__ xyz, in
                 }
                 vs[h].x = kx, vs[h].y = ky, vs[h].z = kz;
                 m.blk[b] = make_int4(kx, ky, kz, 0);
+                if (evidence) evidence[b] = initial;
                 __threadfence();
                 atomicExch((unsigned int *)&m.slots[h].w, b << 8);
                 block = b;
@@ -246,16 +248,21 @@ __global__ void k_mark_far(const int4 *blk, const double *pts, int cap, uint32_t
 }
 
 // `first`: only blocks [first, num_blocks) move; new_id[b] counts the survivors in [first, b), so block b lands at first + new_id[b]
-// (the prefix [0, first) is a frozen prior, which the spare arrays already hold)
+// (the prefix [0, first) is a frozen prior, which the spare arrays already hold).  `ev` / `ev_out` (occupancy on): the blocks'
+// evidence moves with them.
 __global__ void k_compact_blocks(const int4 *blk, const double *pts, int cap, uint32_t num_blocks, const uint32_t *keep,
-                                 const uint32_t *new_id, int4 *blk_out, double *pts_out, uint32_t first = 0) {
+                                 const uint32_t *new_id, int4 *blk_out, double *pts_out, uint32_t first = 0, const int32_t *ev = nullptr,
+                                 int32_t *ev_out = nullptr) {
     // one warp per block: header by lane 0, points copied cooperatively (blocks beyond the live count carry keep = 0)
     const uint32_t b = first + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     const int lane = threadIdx.x & 31;
     if (b >= num_blocks || !keep[b]) return;
     const uint32_t nb = first + new_id[b];
     const int4 h = blk[b];
-    if (lane == 0) blk_out[nb] = h;
+    if (lane == 0) {
+        blk_out[nb] = h;
+        if (ev_out) ev_out[nb] = ev[b];
+    }
     const double *src = pts + (size_t)b * cap * KICP_PSTRIDE;
     double *dst = pts_out + (size_t)nb * cap * KICP_PSTRIDE;
     for (int i = lane; i < h.w * KICP_PSTRIDE; i += 32) dst[i] = src[i];

@@ -25,11 +25,17 @@ __all__ = ["Context", "VoxelHashMap", "Scan", "KinematicRegistration", "KicpErro
            "frame_clouds_device", "PointCloudSensor", "LaserScanSensor", "StageSensors", "StagedSensors", "RegisterStagedSensors",
            "RegisterStagedFrameSegments", "RegisterStagedSensorsSegments", "deskew_segments", "CorrespondenceStats",
            "frame_correspondences", "frame_correspondences_device", "PoseHypothesis", "PlanarAlignment", "frame_map_update",
-           "FreeSpaceStats", "frame_free_space", "FREE_SPACE_MIN_MISSES", "FREE_SPACE_END_MARGIN"]
+           "FreeSpaceStats", "frame_free_space", "FREE_SPACE_MIN_MISSES", "FREE_SPACE_END_MARGIN", "OCCUPANCY_INITIAL",
+           "OCCUPANCY_HIT_GAIN", "OCCUPANCY_MISS_LOSS", "OCCUPANCY_MAX_EVIDENCE"]
 
 # The defaults of free-space clearing (VoxelHashMap.ClearFreeSpace, Context.set_free_space): see README, "Clearing free space"
 FREE_SPACE_MIN_MISSES = 2
 FREE_SPACE_END_MARGIN = 0.5
+# The defaults of occupancy evidence (VoxelHashMap.set_occupancy): see README, "Clearing free space"
+OCCUPANCY_INITIAL = 3
+OCCUPANCY_HIT_GAIN = 1
+OCCUPANCY_MISS_LOSS = 1
+OCCUPANCY_MAX_EVIDENCE = 3
 
 
 class CorrespondenceStats(NamedTuple):
@@ -350,6 +356,27 @@ class VoxelHashMap:
             check(lib().kicp_map_clear_free_space(self.h, dp(q), len(q), dp(pose), dp(o), C.byref(p), C.byref(st)),
                   "kicp_map_clear_free_space")
         return FreeSpaceStats.from_c(st)
+
+    def set_occupancy(self, initial=OCCUPANCY_INITIAL, hit_gain=OCCUPANCY_HIT_GAIN, miss_loss=OCCUPANCY_MISS_LOSS,
+                      max_evidence=OCCUPANCY_MAX_EVIDENCE):
+        """kicp_map_set_occupancy: every live voxel keeps an integer evidence across clearing calls (ClearFreeSpace and the frame
+        path's clearing).  A hit adds hit_gain (up to max_evidence); a call in which the voxel is free subtracts miss_loss, and the
+        voxel is cleared when its evidence reaches 0.  Every voxel, those in the map now included, starts at `initial`.
+        set_occupancy(None) turns it off (memoryless clearing).  The setting belongs to the map: Clear() keeps it."""
+        if initial is None:
+            check(lib().kicp_map_set_occupancy(self.h, None), "kicp_map_set_occupancy")
+            return
+        p = _capi.OccupancyParams(int(initial), int(hit_gain), int(miss_loss), int(max_evidence))
+        check(lib().kicp_map_set_occupancy(self.h, C.byref(p)), "kicp_map_set_occupancy")
+
+    def occupancy(self):
+        """The evidence of every voxel as an np.int32 array aligned with export_voxels() (kicp_map_export_occupancy); raises KicpError
+        when occupancy is off."""
+        V = self.num_voxels()
+        out = np.empty(max(V, 1), dtype=np.int32)
+        n = C.c_int64()
+        check(lib().kicp_map_export_occupancy(self.h, out.ctypes.data_as(_capi.c_ip), V, C.byref(n)), "kicp_map_export_occupancy")
+        return out[: n.value].copy()
 
     def freeze(self):
         """kicp_map_freeze: every voxel now in the map becomes a read-only prior that Update never evicts and AddPoints never writes

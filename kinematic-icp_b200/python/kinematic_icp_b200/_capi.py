@@ -103,6 +103,11 @@ class FreeSpaceStats(C.Structure):
                 ("prior_contradicted", C.c_int64)]
 
 
+class OccupancyParams(C.Structure):
+    """kicp_occupancy_params"""
+    _fields_ = [("initial", C.c_int32), ("hit_gain", C.c_int32), ("miss_loss", C.c_int32), ("max_evidence", C.c_int32)]
+
+
 class FrameInput(C.Structure):
     """kicp_frame_input"""
     _fields_ = [("data", C.c_void_p), ("n", C.c_int64), ("dtype", C.c_int32), ("point_step", C.c_int32), ("offset_x", C.c_int32),
@@ -198,6 +203,8 @@ SYMBOLS = [
     ("kicp_map_clear_free_space", C.c_int, [_P, c_dp, C.c_int64, c_dp, c_dp, C.POINTER(FreeSpaceParams), C.POINTER(FreeSpaceStats)]),
     ("kicp_map_clear_free_space_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp, c_dp,
                                                    C.POINTER(FreeSpaceParams), C.POINTER(FreeSpaceStats)]),
+    ("kicp_map_set_occupancy", C.c_int, [_P, C.POINTER(OccupancyParams)]),
+    ("kicp_map_export_occupancy", C.c_int, [_P, c_ip, C.c_int64, C.POINTER(C.c_int64)]),
     ("kicp_map_nearest", C.c_int, [_P, c_dp, C.c_int64, c_dp, c_dp]),
     ("kicp_map_add_points_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     ("kicp_map_update_device", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_dp]),
